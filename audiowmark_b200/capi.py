@@ -22,6 +22,8 @@ BLOCK_A, BLOCK_B, BLOCK_AB = 0, 1, 2
 SYNC_ENTRY = np.dtype([("frame", "<u2"), ("up", "u1", (30,)), ("down", "u1", (30,))])       # awm_sync_entry
 MIX_ENTRY = np.dtype([("frame", "<u2"), ("up", "u1"), ("down", "u1")])                      # awm_mix_entry
 SEARCH_SCORE = np.dtype([("index", "<u8"), ("raw_quality", "<f8"), ("local_mean", "<f8")])  # awm_search_score
+BATCH_ITEM = np.dtype({"names": ["value_offset", "n_frames", "channels"], "formats": ["<u8", "<u8", "<i4"],
+                       "offsets": [0, 8, 16], "itemsize": 24})                                 # awm_batch_item
 
 EXPORTS = [
     "awm_create", "awm_destroy", "awm_last_error", "awm_launch_count", "awm_stream", "awm_synchronize",
@@ -29,6 +31,7 @@ EXPORTS = [
     "awm_fft_r2c", "awm_fft_c2r", "awm_set_embed_tables", "awm_set_sync_tables", "awm_set_mix_tables",
     "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_decode_blocks", "awm_viterbi",
     "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_is_device_pointer", "awm_speed_scan", "awm_embed_resampled", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_prefetch_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
+    "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch",
 ]
 
 _lib = None
@@ -60,6 +63,14 @@ def _ptr(x):
 
 class AwmError(RuntimeError):
     pass
+
+
+def batch_validate(items, n_values: int) -> str:
+    """awm_batch_validate: '' if every (value_offset, n_frames, channels) item fits a packed buffer of n_values values, else the reason"""
+    it = np.array([tuple(int(v) for v in t) for t in items], BATCH_ITEM)
+    err = ctypes.create_string_buffer(256)
+    rc = load().awm_batch_validate(_ptr(it), ctypes.c_size_t(len(it)), ctypes.c_size_t(n_values), err, ctypes.c_size_t(len(err)))
+    return err.value.decode() if rc else ""
 
 
 class Context:

@@ -12,6 +12,7 @@
 #include <string.h>
 #include "awm_approx_tc.cuh"
 #include "awm_embed_strip.cuh"
+#include "awm_embed_batch.cuh"
 #include "awm_viterbi_pair.cuh"
 
 #include <cuda_runtime.h>
@@ -147,6 +148,8 @@ struct awm_ctx
 
   DevBuf tw, win, synth;             // constant tables
   DevBuf frame_mod; int embed_fpb = 0;
+  DevBuf roles; int roles_fpb = 0, roles_n_coded = 0;         // batched embed: role table of one key
+  DevBuf batch_items, batch_coded;
   KeyTab keys[AWM_MAX_KEYS];
 
   // bound PCM
@@ -360,7 +363,7 @@ awm_destroy (awm_ctx *ctx)
     return;
   cudaSetDevice (ctx->device);
   cudaStreamSynchronize (ctx->stream);
-  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->have, &ctx->q, &ctx->scores, &ctx->a_ud, &ctx->a_cnt, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
+  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->have, &ctx->q, &ctx->scores, &ctx->a_ud, &ctx->a_cnt, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
                      &ctx->cand_start, &ctx->cand_noff, &ctx->r_ud, &ctx->r_cnt, &ctx->rvalid, &ctx->r_ent_ud, &ctx->r_ent_flag, &ctx->tw1024, &ctx->vit_off, &ctx->blk_start, &ctx->D, &ctx->raw,
                      &ctx->vit_raw, &ctx->vit_types, &ctx->vit_delta, &ctx->vit_dec, &ctx->vit_bits, &ctx->vit_err, &ctx->vit_order,
                      &ctx->emb_in, &ctx->emb_out, &ctx->emb_in16, &ctx->emb_out16, &ctx->peaks, &ctx->snr, &ctx->rs_in, &ctx->rs_out, &ctx->rs_jobs, &ctx->pcm_rs,
@@ -566,6 +569,24 @@ awm_set_embed_tables (awm_ctx *ctx, const uint8_t *frame_mod_ab, int frames_per_
   CK (cudaMemcpyAsync (ctx->frame_mod.p, frame_mod_ab, bytes, cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaStreamSynchronize (ctx->stream));
   ctx->embed_fpb = frames_per_block;
+  return 0;
+}
+
+int
+awm_set_embed_roles (awm_ctx *ctx, const uint16_t *roles, int frames_per_block, int n_coded_bits)
+{
+  if (!roles || frames_per_block <= 0 || n_coded_bits <= 0 || n_coded_bits > AWM_ROLE_MAX_INDEX + 1)
+    return fail (ctx, "awm_set_embed_roles: bad arguments");
+  const size_t n = size_t (frames_per_block) * (kMaxBand + 1);
+  for (size_t i = 0; i < n; i++)                         /* k_embed_batch reads coded bits at these indices */
+    if ((roles[i] & AWM_ROLE_MARK) && !(roles[i] & AWM_ROLE_SYNC) && (roles[i] >> AWM_ROLE_SHIFT) >= n_coded_bits)
+      return fail (ctx, "awm_set_embed_roles: role %zu names coded bit %d of %d", i, roles[i] >> AWM_ROLE_SHIFT, n_coded_bits);
+  CK (cudaSetDevice (ctx->device));
+  CK (ctx->roles.reserve (n * sizeof (uint16_t)));
+  CK (cudaMemcpyAsync (ctx->roles.p, roles, n * sizeof (uint16_t), cudaMemcpyHostToDevice, ctx->stream));
+  CK (cudaStreamSynchronize (ctx->stream));
+  ctx->roles_fpb = frames_per_block;
+  ctx->roles_n_coded = n_coded_bits;
   return 0;
 }
 
@@ -1005,7 +1026,7 @@ embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frame
   A.tw = ctx->tw.as<float2>();
   A.win = ctx->win.as<float>();
   A.synth = ctx->synth.as<float>();
-  const size_t smem = fft_smem_bytes (kEmbedWarps) + 3 * kFrame * sizeof (float) + 2 * size_t (kEmbedWarps) * kEdge * sizeof (float2);
+  const size_t smem = kEmbedSmem;
   if (set_smem (ctx, k_embed, smem)) return 1;
   /* stereo audio in a 16-byte aligned buffer streams through k_embed_strip (awm_embed_strip.cuh); AWM_EMBED=tile keeps k_embed */
   const char *env_embed = getenv ("AWM_EMBED");
@@ -1215,6 +1236,174 @@ awm_embed_s16 (awm_ctx *ctx, const int16_t *in, int16_t *out, size_t n_frames, i
                int limiter_block, float limiter_ceiling, double *snr_power)
 {
   return embed_any (ctx, in, out, true, n_frames, channels, first_frame_number, frames_pad_start, water_delta, limiter_block, limiter_ceiling, snr_power);
+}
+
+int
+awm_batch_validate (const awm_batch_item *items, size_t n_items, size_t n_values, char *err, size_t err_cap)
+{
+  auto bad = [&] (size_t i, const char *why)
+    {
+      if (err && err_cap)
+        snprintf (err, err_cap, "batch item %zu: %s", i, why);
+      return 1;
+    };
+  if (n_items && !items)
+    return bad (0, "item list is NULL");
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const awm_batch_item& it = items[i];
+      if (it.channels <= 0)
+        return bad (i, "channels must be >= 1");
+      if (it.n_frames > (n_values - std::min<uint64_t> (it.value_offset, n_values)) / uint64_t (it.channels) || it.value_offset > n_values)
+        return bad (i, "extends past the end of the buffer");
+    }
+  if (err && err_cap)
+    err[0] = 0;
+  return 0;
+}
+
+int
+awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                 const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
+                 double *snr_power)
+{
+  char why[160];
+  if (awm_batch_validate (items, n_items, n_values, why, sizeof (why)))
+    return fail (ctx, "awm_embed_batch: %s", why);
+  if (!ctx->roles_fpb)
+    return fail (ctx, "awm_embed_batch: awm_set_embed_roles has not been called");
+  if ((n_items && !coded_bits) || (n_values && (!in_v || !out_v)))
+    return fail (ctx, "awm_embed_batch: bad arguments");
+  if (snr_power)
+    std::fill (snr_power, snr_power + 2 * n_items, 0.0);
+  if (n_values == 0)
+    return 0;
+  CK (cudaSetDevice (ctx->device));
+  const bool s16 = is_s16 != 0;
+  const bool in_dev = is_device_ptr (in_v), out_dev = is_device_ptr (out_v);
+  /* float images of in / out: the caller's own buffers where they are float device memory, else the context's staging buffers */
+  const float *d_in = !s16 && in_dev ? static_cast<const float *> (in_v) : nullptr;
+  float *d_out = !s16 && out_dev ? static_cast<float *> (out_v) : nullptr;
+  if (!d_in)
+    {
+      CK (ctx->emb_in.reserve (n_values * sizeof (float)));
+      d_in = ctx->emb_in.as<float>();
+    }
+  if (!d_out)
+    {
+      CK (ctx->emb_out.reserve (n_values * sizeof (float)));
+      d_out = ctx->emb_out.as<float>();
+    }
+  const unsigned conv_grid = unsigned (((n_values + 1) / 2 + 255) / 256);
+  if (s16)
+    {
+      const int16_t *d_in16 = static_cast<const int16_t *> (in_v);
+      if (!in_dev)
+        {
+          CK (ctx->emb_in16.reserve (n_values * sizeof (int16_t)));
+          CK (cudaMemcpyAsync (ctx->emb_in16.p, in_v, n_values * sizeof (int16_t), cudaMemcpyHostToDevice, ctx->stream));
+          d_in16 = ctx->emb_in16.as<int16_t>();
+        }
+      PROF (ctx);
+      k_s16_to_f32<<<conv_grid, 256, 0, ctx->stream>>> (d_in16, ctx->emb_in.as<float>(), (long long) n_values);
+      LAUNCH_CHECK ("k_s16_to_f32");
+    }
+  else if (!in_dev)
+    CK (cudaMemcpyAsync (ctx->emb_in.p, in_v, n_values * sizeof (float), cudaMemcpyHostToDevice, ctx->stream));
+
+  /* work list: non-empty items with their first tile, first limiter CTA and block peaks */
+  std::vector<BatchItem> list;
+  long long n_tiles = 0, n_lim = 0, n_peaks = 0;
+  uint64_t covered = 0;
+  for (size_t i = 0; i < n_items; i++)
+    {
+      covered += items[i].n_frames * uint64_t (items[i].channels);
+      if (!items[i].n_frames)
+        continue;
+      BatchItem b;
+      b.v0 = (long long) items[i].value_offset;
+      b.n_frames = (long long) items[i].n_frames;
+      b.C = items[i].channels;
+      b.item = int (i);
+      const long long n_proc = (b.n_frames + kFrame - 1) / kFrame + 1;
+      b.tile0 = n_tiles;
+      b.lim0 = n_lim;
+      b.peak0 = n_peaks;
+      b.n_blocks = limiter_block > 0 ? (n_proc * kFrame + limiter_block - 1) / limiter_block + 2 : 0;   // as awm_embed's
+      n_tiles += (n_proc + kEmbedTile - 1) / kEmbedTile;
+      n_lim += (b.n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter);
+      n_peaks += b.n_blocks;
+      list.push_back (b);
+    }
+  if (n_tiles >= INT_MAX || list.size() >= size_t (INT_MAX))
+    return fail (ctx, "awm_embed_batch: batch too large (%lld tiles)", n_tiles);
+  if (covered < n_values)               /* values between items pass through unchanged */
+    CK (cudaMemcpyAsync (d_out, d_in, n_values * sizeof (float), cudaMemcpyDeviceToDevice, ctx->stream));
+  if (!list.empty())
+    {
+      const size_t coded_bytes = n_items * 2 * size_t (ctx->roles_n_coded);
+      CK (ctx->batch_items.reserve (list.size() * sizeof (BatchItem)));
+      CK (ctx->batch_coded.reserve (coded_bytes));
+      CK (cudaMemcpyAsync (ctx->batch_items.p, list.data(), list.size() * sizeof (BatchItem), cudaMemcpyHostToDevice, ctx->stream));
+      CK (cudaMemcpyAsync (ctx->batch_coded.p, coded_bits, coded_bytes, cudaMemcpyHostToDevice, ctx->stream));
+      if (n_peaks)
+        {
+          CK (ctx->peaks.reserve (n_peaks * sizeof (unsigned)));
+          CK (cudaMemsetAsync (ctx->peaks.p, 0, n_peaks * sizeof (unsigned), ctx->stream));
+        }
+      if (snr_power)
+        {
+          CK (ctx->snr.reserve (2 * n_items * sizeof (double)));
+          CK (cudaMemsetAsync (ctx->snr.p, 0, 2 * n_items * sizeof (double), ctx->stream));
+        }
+      EmbedArgs A = {};
+      A.in = d_in;
+      A.out = d_out;
+      A.fpb = ctx->roles_fpb;
+      A.frame_number0 = 2LL * A.fpb - frames_pad_start;       // first_frame_number 0: every item is a stream of its own
+      A.pow_up = 0.5f * float (-water_delta * 1);
+      A.pow_down = 0.5f * float (-water_delta * -1);
+      A.limiter_block = limiter_block;
+      A.peaks = ctx->peaks.as<unsigned>();
+      A.snr = snr_power ? ctx->snr.as<double>() : nullptr;
+      A.snr_pos1 = LLONG_MAX;
+      A.tw = ctx->tw.as<float2>();
+      A.win = ctx->win.as<float>();
+      A.synth = ctx->synth.as<float>();
+      const BatchItem *d_items = ctx->batch_items.as<BatchItem>();
+      if (set_smem (ctx, k_embed_batch, kEmbedBatchSmem)) return 1;
+      PROF (ctx);
+      k_embed_batch<<<unsigned (n_tiles), kEmbedWarps * 32, kEmbedBatchSmem, ctx->stream>>> (A, d_items, int (list.size()), ctx->roles.as<uint16_t>(),
+                                                                                            ctx->batch_coded.as<uint8_t>(), ctx->roles_n_coded);
+      LAUNCH_CHECK ("k_embed_batch");
+      if (limiter_block > 0)
+        {
+          PROF (ctx);
+          k_limiter_batch<<<unsigned (n_lim), 256, 0, ctx->stream>>> (d_out, d_items, int (list.size()), limiter_block, limiter_ceiling, ctx->peaks.as<unsigned>());
+          LAUNCH_CHECK ("k_limiter_batch");
+        }
+    }
+  if (s16)
+    {
+      int16_t *d_out16 = static_cast<int16_t *> (out_v);
+      if (!out_dev)
+        {
+          CK (ctx->emb_out16.reserve (n_values * sizeof (int16_t)));
+          d_out16 = ctx->emb_out16.as<int16_t>();
+        }
+      PROF (ctx);
+      k_f32_to_s16<<<conv_grid, 256, 0, ctx->stream>>> (d_out, d_out16, (long long) n_values);
+      LAUNCH_CHECK ("k_f32_to_s16");
+      if (!out_dev)
+        CK (cudaMemcpyAsync (out_v, d_out16, n_values * sizeof (int16_t), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+  else if (!out_dev)
+    CK (cudaMemcpyAsync (out_v, d_out, n_values * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
+  if (snr_power && !list.empty())
+    CK (cudaMemcpyAsync (snr_power, ctx->snr.p, 2 * n_items * sizeof (double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (!out_dev || snr_power)
+    CK (cudaStreamSynchronize (ctx->stream));
+  return 0;
 }
 
 /* ---------------------------------------------------------------- sync search */

@@ -44,11 +44,12 @@ fft_smem_setup (unsigned char *smem, const float2 *g_tw, const float *g_win, int
 
 // load (and window) one pair of real sequences: re <- channel chA, im <- channel chB (or 0)
 // from interleaved PCM, sample-frames [start, start+1024), zero beyond n_frames.
-__device__ __forceinline__ void
+// VEC2: stereo frames are read as float2 (pcm must be 8-byte aligned); false reads single floats, same values.
+template<bool VEC2 = true> __device__ __forceinline__ void
 load_pair (const float *__restrict__ pcm, long long n_frames, int C, long long start, int chA, int chB,
            const float *win, float (&re)[32], float (&im)[32], int lane)
 {
-  if (C == 2 && chB == 1 && start >= 0 && start + kFrame <= n_frames)
+  if (VEC2 && C == 2 && chB == 1 && start >= 0 && start + kFrame <= n_frames)
     {
       /* common case: whole stereo frame inside the buffer -> one base pointer, immediate offsets, no bounds tests */
       const float2 *p = reinterpret_cast<const float2 *> (pcm) + start + lane;
@@ -61,7 +62,7 @@ load_pair (const float *__restrict__ pcm, long long n_frames, int C, long long s
           im[j] = __fmul_rn (v.y, w);
         }
     }
-  else if (C == 2 && chB == 1)
+  else if (VEC2 && C == 2 && chB == 1)
     {
       const float2 *p2 = reinterpret_cast<const float2 *> (pcm);
 #pragma unroll
@@ -915,10 +916,14 @@ embed_mod_group (const float (&re)[32], const float (&im)[32], float (&inr)[32],
   else           { inr[31 - K2] = gi; ini[31 - K2] = gr; }
 }
 
-__global__ void __launch_bounds__ (kEmbedWarps * 32, 1)
-k_embed (EmbedArgs A)
+constexpr size_t kEmbedSmem = fft_smem_bytes (kEmbedWarps) + 3 * kFrame * sizeof (float) + 2 * size_t (kEmbedWarps) * kEdge * sizeof (float2);
+
+// one CTA of k_embed: output frames [tile_first, tile_first + kEmbedTile) of the buffer A describes.  fm_row (r) returns the
+// 101-byte frame-mod row of table row r (0 keep, 1 up, 2 down); the whole warp calls it together.  VEC2: stereo in / out are
+// accessed as float2 (both 8-byte aligned); false uses single floats, with identical results.
+template<bool VEC2, class FmRow> __device__ __forceinline__ void
+embed_tile (const EmbedArgs& A, long long tile_first, unsigned char *smem, FmRow fm_row)
 {
-  extern __shared__ __align__ (16) unsigned char smem[];
   FftSmem s = fft_smem_setup (smem, A.tw, A.win, kEmbedWarps);
   float *synth = s.extra;                                   // [3072]
   float2 *elo = reinterpret_cast<float2 *> (synth + 3 * kFrame);  // [warps][kEdge]   samples x < kEdge
@@ -926,7 +931,7 @@ k_embed (EmbedArgs A)
   for (int i = threadIdx.x; i < 3 * kFrame; i += blockDim.x)
     synth[i] = A.synth[i];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const long long m = A.frame_begin + (long long) blockIdx.x * kEmbedTile - 1 + w;      // frame handled by this warp
+  const long long m = tile_first - 1 + w;                   // frame handled by this warp
   const long long n_real = (A.n_frames + kFrame - 1) / kFrame;          // frames that contain input
   const bool exists = m >= 0 && m < n_real;
   const bool emits = w >= 1 && w <= kEmbedTile && m >= A.frame_begin && m < A.frame_end && m < A.n_proc;
@@ -949,10 +954,10 @@ k_embed (EmbedArgs A)
       __syncthreads();                                      // synth[] ready / previous pair's edges consumed
       if (exists)
         {
-          load_pair (A.in, A.n_frames, C, m * kFrame, chA, chB, s.win, re, im, lane);
+          load_pair<VEC2> (A.in, A.n_frames, C, m * kFrame, chA, chB, s.win, re, im, lane);
           fft1024_warp (re, im, s.tw, s.xbuf, lane);
           const long long r = (A.frame_number0 + m) % (2LL * A.fpb);
-          const uint8_t *fm = A.frame_mod + (size_t) r * (kMaxBand + 1);   // rows [0,fpb) = A, [fpb,2fpb) = B
+          const uint8_t *fm = fm_row (r);                   // rows [0,fpb) = A, [fpb,2fpb) = B
           float inr[32], ini[32];
 #pragma unroll
           for (int j = 0; j < 32; j++)
@@ -1013,7 +1018,7 @@ k_embed (EmbedArgs A)
               float oa = 0.f, ob = 0.f;
               if (pos < A.n_frames)
                 {
-                  if (C == 2)
+                  if (VEC2 && C == 2)
                     {
                       const float2 v = __ldg (reinterpret_cast<const float2 *> (A.in) + pos);
                       oa = v.x; ob = v.y;
@@ -1037,7 +1042,7 @@ k_embed (EmbedArgs A)
               if (x < boundary) pk0 = fmaxf (pk0, mx); else pk1 = fmaxf (pk1, mx);
               if (pos < A.n_frames)
                 {
-                  if (C == 2)
+                  if (VEC2 && C == 2)
                     reinterpret_cast<float2 *> (A.out)[pos] = make_float2 (ya, yb);
                   else
                     {
@@ -1080,15 +1085,23 @@ k_embed (EmbedArgs A)
     }
 }
 
+__global__ void __launch_bounds__ (kEmbedWarps * 32, 1)
+k_embed (EmbedArgs A)
+{
+  extern __shared__ __align__ (16) unsigned char smem[];
+  embed_tile<true> (A, A.frame_begin + (long long) blockIdx.x * kEmbedTile, smem,
+                    [&] (long long r) { return A.frame_mod + (size_t) r * (kMaxBand + 1); });
+}
+
 // Limiter::process_block (src/limiter.cc:99-124): gain ramps linearly over each block between
 // ceiling / max (bm[b-1], bm[b]) and ceiling / max (bm[b], bm[b+1]); bm[b] = max (ceiling, peak[b]).
 constexpr int kLimiterIter = 16;        // sample-frames per thread: a CTA covers 4096 consecutive positions
 
-__global__ void
-k_limiter (float *__restrict__ x, long long pos_begin, long long pos_end, int C, int block, float ceiling,
-           const unsigned *__restrict__ peaks, long long n_blocks, long long stream_pos0)
+// one CTA of k_limiter: positions [cta_first, cta_first + blockDim.x * kLimiterIter) clipped to pos_end
+__device__ __forceinline__ void
+limiter_cta (float *__restrict__ x, long long cta_first, long long pos_end, int C, int block, float ceiling,
+             const unsigned *__restrict__ peaks, long long n_blocks, long long stream_pos0)
 {
-  const long long cta_first = pos_begin + (long long) blockIdx.x * blockDim.x * kLimiterIter;
   if (cta_first >= pos_end)
     return;
   // most audio never reaches the ceiling: if no limiter block that touches this CTA's range (or its neighbours, which steer the
@@ -1124,6 +1137,13 @@ k_limiter (float *__restrict__ x, long long pos_begin, long long pos_end, int C,
       for (int c = 0; c < C; c++)
         x[pos * C + c] = __fmul_rn (x[pos * C + c], scale);
     }
+}
+
+__global__ void
+k_limiter (float *__restrict__ x, long long pos_begin, long long pos_end, int C, int block, float ceiling,
+           const unsigned *__restrict__ peaks, long long n_blocks, long long stream_pos0)
+{
+  limiter_cta (x, pos_begin + (long long) blockIdx.x * blockDim.x * kLimiterIter, pos_end, C, block, ceiling, peaks, n_blocks, stream_pos0);
 }
 
 } // namespace awm

@@ -13,6 +13,9 @@ std::vector<SlotInfo> g_slots;
 std::vector<unsigned char> g_embed_key;
 std::vector<int>           g_embed_bits;
 int                        g_embed_fpb_mix = -1;
+/* the role table currently on the device (batched embed) */
+SlotInfo                   g_roles;
+bool                       g_roles_valid = false;
 }
 
 awm_ctx *
@@ -42,6 +45,7 @@ Engine::shutdown()
   g_slots.clear();
   g_embed_key.clear();
   g_embed_bits.clear();
+  g_roles_valid = false;
 }
 
 std::string
@@ -103,6 +107,8 @@ Engine::set_embed_tables (const Key& key, const std::vector<int>& bitvec)
   if (kb == g_embed_key && bitvec == g_embed_bits && sig == g_embed_fpb_mix)
     return true;                                  // same key + payload as the previous `add`: table is already uploaded
   const std::vector<uint8_t> fm = gen_frame_mod_ab (key, bitvec);
+  if (fm.empty())
+    return false;
   if (awm_set_embed_tables (c, fm.data(), int (frames_per_block())))
     {
       error ("audiowmark: %s\n", awm_last_error (c));
@@ -111,6 +117,30 @@ Engine::set_embed_tables (const Key& key, const std::vector<int>& bitvec)
   g_embed_key = kb;
   g_embed_bits = bitvec;
   g_embed_fpb_mix = sig;
+  return true;
+}
+
+bool
+Engine::set_embed_roles (const Key& key)
+{
+  awm_ctx *c = ctx();
+  if (!c)
+    return false;
+  const std::vector<unsigned char> kb (key.aes_key(), key.aes_key() + Key::SIZE);
+  const SlotInfo sig { kb, Params::payload_size, Params::frames_per_bit, Params::mix };
+  if (g_roles_valid && g_roles.key == sig.key && g_roles.payload_size == sig.payload_size && g_roles.frames_per_bit == sig.frames_per_bit &&
+      g_roles.mix == sig.mix)
+    return true;                                  // same key and layout as the previous batch: roles are already uploaded
+  const std::vector<uint16_t> roles = gen_embed_roles (key);
+  if (roles.empty())
+    return false;
+  if (awm_set_embed_roles (c, roles.data(), int (frames_per_block()), int (code_size (ConvBlockType::a, Params::payload_size))))
+    {
+      error ("audiowmark: %s\n", awm_last_error (c));
+      return false;
+    }
+  g_roles = sig;
+  g_roles_valid = true;
   return true;
 }
 

@@ -16,6 +16,7 @@ public:
   static void     shutdown();
   static int      key_slot (const Key& key);   // uploads sync (BLOCK + CLIP) and mix tables on first use; -1 on error
   static bool     set_embed_tables (const Key& key, const std::vector<int>& bitvec);
+  static bool     set_embed_roles (const Key& key);    // role table of the batched embed, uploaded once per key / layout
   static std::string last_error();
   static bool     is_device_pointer (const void *p);   // true if p is CUDA device (or managed) memory
 };

@@ -175,10 +175,34 @@ awmh_frame_mod (const unsigned char *key16, const char *payload_hex, uint8_t *ou
   if (bitvec.empty())
     return -1;
   const std::vector<uint8_t> fm = gen_frame_mod_ab (make_key (key16, ""), bitvec);
-  if (fm.size() > out_size)
+  if (fm.empty() || fm.size() > out_size)
     return -1;
   memcpy (out, fm.data(), fm.size());
   return int (fm.size());
+}
+
+/* the two halves of gen_frame_mod_ab: key-only role codes [frames_per_block][101] and one payload's coded bits [2][n_coded] */
+int
+awmh_embed_roles (const unsigned char *key16, uint16_t *out, size_t out_size)
+{
+  const std::vector<uint16_t> roles = gen_embed_roles (make_key (key16, ""));
+  if (roles.empty() || roles.size() > out_size)
+    return -1;
+  memcpy (out, roles.data(), roles.size() * sizeof (uint16_t));
+  return int (roles.size());
+}
+
+int
+awmh_coded_bits (const unsigned char *key16, const char *payload_hex, uint8_t *out, size_t out_size)
+{
+  const std::vector<int> bitvec = parse_payload (payload_hex);
+  if (bitvec.empty())
+    return -1;
+  const std::vector<uint8_t> coded = gen_coded_bits (make_key (key16, ""), bitvec);
+  if (coded.size() > out_size)
+    return -1;
+  memcpy (out, coded.data(), coded.size());
+  return int (coded.size());
 }
 
 int
@@ -234,6 +258,42 @@ awmh_add (const unsigned char *key16, const float *in, float *out, size_t n_fram
   if (snr_db)
     *snr_db = stats.snr_db;
   return rc;
+}
+
+/* add_watermark_batch on a packed buffer (float or 16 bit PCM, host or device): payload_hex[i] goes into items[i];
+ * data_blocks / snr_db (optional): [n_items].  Returns 2 for a malformed item list (checked before any GPU work). */
+static int
+add_batch_any (const unsigned char *key16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+               const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
+{
+  std::vector<std::string> bits (n_items);
+  for (size_t i = 0; i < n_items; i++)
+    bits[i] = payload_hex[i] ? payload_hex[i] : "";
+  std::vector<AddStats> stats;
+  const int rc = add_watermark_batch (make_key (key16, ""), in, out, s16, n_values, items, n_items, bits, sample_rate,
+                                      (data_blocks || snr_db) ? &stats : nullptr);
+  for (size_t i = 0; i < stats.size(); i++)
+    {
+      if (data_blocks)
+        data_blocks[i] = stats[i].data_blocks;
+      if (snr_db)
+        snr_db[i] = stats[i].snr_db;
+    }
+  return rc;
+}
+
+int
+awmh_add_batch (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
+{
+  return add_batch_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db);
+}
+
+int
+awmh_add_batch_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                    const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
+{
+  return add_batch_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db);
 }
 
 /* add / get between 16 bit PCM host buffers (the contents of a 16 bit WAV file): conversions run on the device */

@@ -1,6 +1,7 @@
 #include "awm_tables.hh"
 #include "awm_params.hh"
 #include "awm_util.hh"
+#include "../csrc/awm_roles.hh"
 
 #include <algorithm>
 #include <assert.h>
@@ -76,6 +77,21 @@ bit_order (const Key& key, size_t n)
   return order;
 }
 
+/* bit_order of the last key asked for: a batch encodes every payload with the same key */
+static const std::vector<unsigned>&
+cached_bit_order (const Key& key, size_t n)
+{
+  static std::vector<unsigned char> c_key;
+  static std::vector<unsigned> c_order;
+  const std::vector<unsigned char> kb (key.aes_key(), key.aes_key() + Key::SIZE);
+  if (kb != c_key || c_order.size() != n)
+    {
+      c_order = bit_order (key, n);
+      c_key = kb;
+    }
+  return c_order;
+}
+
 SyncTable
 gen_sync_table (const Key& key, int mode)
 {
@@ -116,55 +132,76 @@ gen_sync_table (const Key& key, int mode)
   return tab;
 }
 
+std::vector<uint16_t>
+gen_embed_roles (const Key& key)
+{
+  const size_t fpb = frames_per_block(), n_bins = Params::max_band + 1;
+  std::vector<uint16_t> roles (fpb * n_bins, 0);
+  bool collision = false;
+  /* an up band carries the bit, a down band its inverse (init_frame_mod_vec, src/wmadd.cc:61-84) */
+  auto set = [&] (int frame, int bin, bool down, bool sync, int index)
+    {
+      uint16_t& r = roles[frame * n_bins + bin];
+      collision |= r != 0;
+      r = AWM_ROLE_MARK | (down ? AWM_ROLE_DOWN : 0) | (sync ? AWM_ROLE_SYNC : 0) | (index << AWM_ROLE_SHIFT);
+    };
+  BitPosGen bit_pos_gen (key);
+  UpDownGen sync_gen (key, Random::Stream::sync_up_down);
+  for (int f = 0; f < int (mark_sync_frame_count()); f++)
+    {
+      UpDownArray up, down;
+      sync_gen.get (f, up, down);
+      for (size_t i = 0; i < up.size(); i++)
+        {
+          set (bit_pos_gen.sync_frame (f), up[i], false, true, f / Params::sync_frames_per_bit);
+          set (bit_pos_gen.sync_frame (f), down[i], true, true, f / Params::sync_frames_per_bit);
+        }
+    }
+  /* data frames: with mixing the coded bit of an entry follows from its position after the shuffle, not from its frame */
+  const std::vector<MixEntry> entries = gen_mix_entries (key);
+  for (size_t e = 0; e < entries.size(); e++)
+    {
+      const int bit = e / Params::bands_per_frame / Params::frames_per_bit;
+      set (entries[e].frame, entries[e].up, false, false, bit);
+      set (entries[e].frame, entries[e].down, true, false, bit);
+    }
+  if (collision)
+    {
+      /* sync and data frames are distinct positions of one BitPosGen permutation and up / down bands of a frame are disjoint,
+       * so no entry can carry two bits; a table that does would not embed what the reference embeds */
+      error ("audiowmark: embed roles: a (frame, bin) entry is assigned twice\n");
+      return {};
+    }
+  return roles;
+}
+
+std::vector<uint8_t>
+gen_coded_bits (const Key& key, const std::vector<int>& bitvec)
+{
+  std::vector<uint8_t> out;
+  for (ConvBlockType t : { ConvBlockType::a, ConvBlockType::b })
+    {
+      const std::vector<int> coded = code_encode (t, bitvec);
+      const std::vector<unsigned>& order = cached_bit_order (key, coded.size());
+      for (size_t i = 0; i < coded.size(); i++)
+        out.push_back (coded[order[i]]);                  // randomize_bit_order (encode)
+    }
+  return out;
+}
+
 std::vector<uint8_t>
 gen_frame_mod_ab (const Key& key, const std::vector<int>& bitvec)
 {
-  enum { KEEP = 0, UP = 1, DOWN = 2 };
   const size_t fpb = frames_per_block(), n_bins = Params::max_band + 1;
-  std::vector<uint8_t> tab (2 * fpb * n_bins, KEEP);
-  const std::vector<MixEntry> mix_entries = Params::mix ? gen_mix_entries (key) : std::vector<MixEntry>();
-  BitPosGen bit_pos_gen (key);
+  const std::vector<uint16_t> roles = gen_embed_roles (key);
+  if (roles.empty())
+    return {};
+  const std::vector<uint8_t> coded = gen_coded_bits (key, bitvec);
+  const size_t n_coded = coded.size() / 2;
+  std::vector<uint8_t> tab (2 * fpb * n_bins);
   for (int ab = 0; ab < 2; ab++)
-    {
-      uint8_t *fm = &tab[ab * fpb * n_bins];
-      auto mark = [&] (int frame, const UpDownArray& up, const UpDownArray& down, int data_bit)
-        {
-          for (int u : up)   fm[frame * n_bins + u] = data_bit ? UP : DOWN;
-          for (int d : down) fm[frame * n_bins + d] = data_bit ? DOWN : UP;
-        };
-      const std::vector<int> fec = randomize_bit_order (key, code_encode (ab ? ConvBlockType::b : ConvBlockType::a, bitvec), /* encode */ true);
-      /* sync frames: 010101 for A, 101010 for B, written in linear order */
-      UpDownGen sync_gen (key, Random::Stream::sync_up_down);
-      for (int f = 0; f < int (mark_sync_frame_count()); f++)
-        {
-          UpDownArray up, down;
-          sync_gen.get (f, up, down);
-          mark (bit_pos_gen.sync_frame (f), up, down, (f / Params::sync_frames_per_bit + ab) & 1);
-        }
-      /* data frames */
-      const int data_frames = mark_data_frame_count();
-      if (Params::mix)
-        {
-          for (int f = 0; f < data_frames; f++)
-            for (size_t fb = 0; fb < Params::bands_per_frame; fb++)
-              {
-                const MixEntry& me = mix_entries[f * Params::bands_per_frame + fb];
-                const int data_bit = fec[f / Params::frames_per_bit];
-                fm[me.frame * n_bins + me.up]   = data_bit ? UP : DOWN;
-                fm[me.frame * n_bins + me.down] = data_bit ? DOWN : UP;
-              }
-        }
-      else
-        {
-          UpDownGen data_gen (key, Random::Stream::data_up_down);
-          for (int f = 0; f < data_frames; f++)
-            {
-              UpDownArray up, down;
-              data_gen.get (f, up, down);
-              mark (bit_pos_gen.data_frame (f), up, down, fec[f / Params::frames_per_bit]);
-            }
-        }
-    }
+    for (size_t i = 0; i < fpb * n_bins; i++)
+      tab[ab * fpb * n_bins + i] = role_frame_mod (roles[i], ab, &coded[ab * n_coded]);
   return tab;
 }
 

@@ -55,7 +55,12 @@ struct SyncTable            // get_sync_bits flattened bit-major for awm_set_syn
 };
 SyncTable gen_sync_table (const Key& key, int mode /* AWM_MODE_* */);
 
-/* FrameMod table [2][frames_per_block][101] for awm_set_embed_tables: 0 keep, 1 up, 2 down */
+/* role table [frames_per_block][101] for awm_set_embed_roles (codes: include/awm_b200.h); empty (with an error message) if an
+ * entry would be assigned twice */
+std::vector<uint16_t> gen_embed_roles (const Key& key);
+/* coded data bits [2 (A, B)][n_coded] of one payload: randomize_bit_order (code_encode (A | B, bitvec)) */
+std::vector<uint8_t> gen_coded_bits (const Key& key, const std::vector<int>& bitvec);
+/* FrameMod table [2][frames_per_block][101] for awm_set_embed_tables: 0 keep, 1 up, 2 down; roles x coded bits (empty on error) */
 std::vector<uint8_t> gen_frame_mod_ab (const Key& key, const std::vector<int>& bitvec);
 
 std::vector<int> parse_payload (const std::string& bits);   // src/wmcommon.cc:210-238

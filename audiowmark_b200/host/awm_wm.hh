@@ -19,6 +19,12 @@ struct AddStats { int data_blocks = 0; double snr_db = 0; };
 int add_watermark_buffer (const Key& key, const float *in, float *out, size_t n_frames, int n_channels, int sample_rate,
                           const std::string& bits, AddStats *stats, uint64_t first_frame_number = 0);
 
+/* add_watermark_buffer for many items of one packed buffer (float or 16 bit PCM, host or device), one payload per item, in one pass
+ * over the GPU; item i comes out bit identical to add_watermark_buffer[_s16] on it alone.  44.1 kHz only.  stats (optional) gets
+ * one entry per item.  Returns 2 for a malformed item list or payload, 1 for other errors. */
+int add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                         const std::vector<std::string>& bits, int sample_rate, std::vector<AddStats> *stats);
+
 /* add_stream_watermark's loop with bounded memory (window by window; see awm_add.cc); callbacks read / write interleaved frames */
 int add_watermark_windowed (const Key& key, const std::function<Error (std::vector<float>&, size_t)>& read,
                             const std::function<Error (const std::vector<float>&)>& write, int n_channels, int sample_rate, const std::string& bits,

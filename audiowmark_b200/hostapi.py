@@ -16,7 +16,8 @@ LIB_PATH = os.path.join(_HERE, "lib", "libawm_host.so")
 CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
-           "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_add_windowed"]
+           "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_add_windowed",
+           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16"]
 
 _lib = None
 
@@ -121,6 +122,23 @@ def frame_mod(key, payload_hex: str) -> np.ndarray:
     return out
 
 
+def embed_roles(key) -> np.ndarray:
+    """key-only role codes uint16 [frames_per_block, 101] of the FrameMod table (codes: include/awm_b200.h)"""
+    out = np.zeros((frames_per_block(), 101), np.uint16)
+    n = load().awmh_embed_roles(_key(key), _ptr(out), ctypes.c_size_t(out.size))
+    assert n == out.size
+    return out
+
+
+def coded_bits(key, payload_hex: str) -> np.ndarray:
+    """one payload's coded data bits uint8 [2 (A, B), n_coded]: randomize_bit_order (code_encode (A | B, payload))"""
+    out = np.zeros((2, n_coded_bits()), np.uint8)
+    n = load().awmh_coded_bits(_key(key), payload_hex.encode(), _ptr(out), ctypes.c_size_t(out.size))
+    if n != out.size:
+        raise ValueError("cannot encode payload %r" % payload_hex)
+    return out
+
+
 def conv_encode(block_type: int, bits) -> np.ndarray:
     b = np.ascontiguousarray(bits, np.uint8)
     out = np.zeros((len(b) + 15) * 12, np.uint8)
@@ -162,6 +180,59 @@ def add(pcm_in, payload_hex: str, key=None, pcm_out=None, n_frames=None, channel
     if rc:
         raise RuntimeError("awmh_add failed (rc=%d); see stderr" % rc)
     return (pcm_out, blocks.value, snr.value) if want_stats else pcm_out
+
+
+def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False):
+    """`add` for many items with one key and one payload each, in one pass over the GPU; item i comes out bit identical to
+    add / add_s16 of that item alone with payloads[i].
+      pcms: a list of numpy arrays [n, channels] (all float32 or all int16; channels may differ), or one packed device tensor
+            (float32 or int16, contiguous) with items = [(value_offset, n_frames, channels), ...] in values of that tensor;
+            out: a device tensor like pcms for the result (default: a new one).
+    Returns the list of outputs (numpy arrays, or views of the output tensor), with want_stats also the lists of data blocks
+    and SNR dB per item.  Only 44.1 kHz input is accepted.  Raises ValueError for a malformed item list or payload."""
+    payloads = list(payloads)
+    if items is None:
+        arrays = [np.asarray(p) for p in pcms]
+        s16 = bool(arrays) and all(a.dtype == np.int16 for a in arrays)
+        dt = np.int16 if s16 else np.float32
+        arrays = [a.reshape(-1, 1) if a.ndim == 1 else a for a in arrays]
+        items = []
+        off = 0
+        for a in arrays:
+            items.append((off, a.shape[0], a.shape[1]))
+            off += a.size
+        packed = np.concatenate([np.ascontiguousarray(a, dt).reshape(-1) for a in arrays]) if arrays else np.zeros(0, dt)
+        res = np.empty_like(packed)
+        n_values, p_in, p_out = packed.size, _ptr(packed), _ptr(res)
+        split = lambda o, n, c: res[o:o + n * c].reshape(n, c)
+    else:
+        import torch
+        if not (pcms.is_cuda and pcms.is_contiguous() and pcms.dtype in (torch.float32, torch.int16)):
+            raise ValueError("add_batch: pcms must be a contiguous float32 or int16 CUDA tensor")
+        s16 = pcms.dtype == torch.int16
+        res = torch.empty_like(pcms) if out is None else out
+        if res.dtype != pcms.dtype or res.numel() != pcms.numel() or not res.is_contiguous():
+            raise ValueError("add_batch: out must be a contiguous tensor like pcms")
+        flat = res.view(-1)
+        torch.cuda.current_stream(pcms.device).synchronize()      # the context works on its own stream
+        n_values, p_in, p_out = pcms.numel(), ctypes.c_void_p(pcms.data_ptr()), ctypes.c_void_p(res.data_ptr())
+        split = lambda o, n, c: flat[o:o + n * c].view(n, c)
+    if len(payloads) != len(items):
+        raise ValueError("add_batch: %d items but %d payloads" % (len(items), len(payloads)))
+    it = np.array([tuple(int(v) for v in t) for t in items], capi.BATCH_ITEM)
+    pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
+    blocks = np.zeros(max(len(it), 1), np.int32)
+    snr = np.zeros(max(len(it), 1), np.float64)
+    fn = load().awmh_add_batch_s16 if s16 else load().awmh_add_batch
+    rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, ctypes.c_int(sample_rate),
+            _ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
+    if rc == 2:
+        raise ValueError("add_batch: malformed item list or payload; see stderr")
+    if rc:
+        raise RuntimeError("awmh_add_batch failed (rc=%d); see stderr" % rc)
+    synchronize()
+    outs = [split(int(t["value_offset"]), int(t["n_frames"]), int(t["channels"])) for t in it]
+    return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs
 
 
 def add_windowed(pcm_in: np.ndarray, payload_hex: str, key=None, zero_frames=0, window_frames=0, sample_rate=44100):

@@ -154,6 +154,41 @@ int awm_embed_s16 (awm_ctx *ctx, const int16_t *in, int16_t *out, size_t n_frame
                    uint64_t first_frame_number, int frames_pad_start, double water_delta,
                    int limiter_block, float limiter_ceiling, double *snr_power);
 
+/* ---- batched embed: many items, one key, one payload per item ------------------------------------------------
+ * The FrameMod table of one (key, payload) is a key-only ROLE per (frame, bin) combined with the payload's coded bits.
+ * Role code (uint16): 0 = keep; otherwise bit 0 is set, bit 1 = down band (the bit is inverted), bit 2 = sync bit,
+ * bits 3..15 = index: of a coded data bit (data frames, position after randomize_bit_order) or of a sync bit.
+ * The bit of a role in block ab (0 = A, 1 = B) is coded[ab][index] for data, (index + ab) & 1 for sync
+ * (sync frames carry 010101 in A blocks, 101010 in B blocks); 1 -> entry 1 (up), 0 -> entry 2 (down), after the inversion. */
+#define AWM_ROLE_MARK   1
+#define AWM_ROLE_DOWN   2
+#define AWM_ROLE_SYNC   4
+#define AWM_ROLE_SHIFT  3
+#define AWM_ROLE_MAX_INDEX 8191
+
+/* one item of a batch: n_frames sample-frames of `channels` interleaved channels starting at value value_offset of the
+ * packed buffer (values, not frames: items of different channel counts share one buffer) */
+typedef struct {
+  uint64_t value_offset;
+  uint64_t n_frames;
+  int      channels;
+} awm_batch_item;
+
+/* role table uint16 [frames_per_block][101] of one key; n_coded_bits = coded data bits per block (every data index < it) */
+int awm_set_embed_roles (awm_ctx *ctx, const uint16_t *roles, int frames_per_block, int n_coded_bits);
+/* 0 if every item has channels >= 1 and lies inside a packed buffer of n_values values, else nonzero with the reason in err
+ * (err may be NULL).  Needs no device; awm_embed_batch runs the same check. */
+int awm_batch_validate (const awm_batch_item *items, size_t n_items, size_t n_values, char *err, size_t err_cap);
+/* awm_embed (first_frame_number 0) for every item of a packed buffer in one pass: item i comes out bit identical to awm_embed /
+ * awm_embed_s16 on that item alone with the FrameMod table of payload i.  in / out: n_values floats (is_s16 = 0) or int16
+ * (is_s16 = 1), host or device; host buffers cross PCIe as one copy each way.  Items must not overlap.  Values of out that belong
+ * to no item are copied from in when out is host memory and left alone when it is device memory.
+ * coded_bits: uint8 [n_items][2 (A, B)][n_coded_bits] (randomize_bit_order (code_encode (A | B, payload))).
+ * snr_power (optional): [n_items][2] as awm_embed's.  Roles come from awm_set_embed_roles; zero items and zero-length items are legal. */
+int awm_embed_batch (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                     const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
+                     double *snr_power);
+
 /* ---- sync search on the bound PCM --------------------------------------------------------
  * awm_sync_approx = SyncFinder::search_approx (src/syncfinder.cc:171-256): for the four
  * 256-sample shifts the channel-summed dB spectrogram (sync_fft, :560-605), sync_decode (:116-153)
