@@ -9,13 +9,13 @@
 //   * A operand = the dB tile, written by the FFT warps straight into the K-major operand layout (awm_tc.cuh) as TWO fp16 terms
 //     hi = fp16 (v), lo = fp16 (v - hi): |v| < 256, so hi + lo carries v to 2^-16 absolute -- the resolution fp32 itself has there;
 //     every product with a 0/1 mask element is exact, accumulation is fp32
-//   * B operand = the 0/1 masks of CHUNK_ENT entries (2 CHUNK_ENT columns: U and D of an entry side by side), prepared once per key
-//     on the host in operand layout and fetched chunk by chunk with the bulk-copy engine (TMA, cp.async.bulk -> mbarrier complete_tx)
+//   * B operand = the 0/1 masks of 48 entries (96 columns: U and D of an entry side by side), prepared once per key on the host in
+//     operand layout and fetched chunk by chunk with the bulk-copy engine (TMA, cp.async.bulk -> mbarrier complete_tx)
 //   * D = 64 x 32 fp32 blocks in the registers of the MMA warpgroup, which writes them to `mags` itself
 // Warp roles (one CTA per SM, CTAs walk the (frame tile, shift) list with stride gridDim.x):
-//   warps 0 .. F-1     FFT: frame (PCM prefetched by TMA into the warp's transpose buffer) -> packed 1024-point FFT -> dB ->
+//   warps 0 .. 11      FFT: frame (PCM prefetched by TMA into the warp's transpose buffer) -> packed 1024-point FFT -> dB ->
 //                      fp16 hi/lo into A[buf]                                                     (a_empty -> a_full)
-//   warps F .. F+3     one warpgroup: B chunk loads (thread 0), wgmma per 64 x 32 block, stores   (a_full, b_full -> a_empty)
+//   warps 12 .. 15     one warpgroup: B chunk loads (thread 0), wgmma per 64 x 32 block, stores   (a_full, b_full -> a_empty)
 // All hand-offs are mbarriers; the FFT of tile i + 1 overlaps the MMAs and the stores of tile i.
 #pragma once
 #include "awm_kernels.cuh"
@@ -30,48 +30,47 @@ constexpr uint32_t kTcASplit = kTcTile * kTcK * 2;        // bytes of one fp16 t
 constexpr uint32_t kTcABytes = 2 * kTcASplit;             // hi + lo
 constexpr int kTcEpiWarps = 4;             // the MMA warpgroup
 constexpr int kTcNB = 32;                  // columns (16 entries) per wgmma block
-// CHUNK_ENT sync entries per B chunk -> N = 2 CHUNK_ENT columns (U and D column of every entry), chunk of N x 96 fp16.
-// 128 entries (N = 256, 48 KB) with eight FFT warps; 48 entries (N = 96, 18 KB) leave room for twelve FFT warps AND two A buffers.
-__host__ __device__ constexpr uint32_t tc_b_bytes (int chunk_ent) { return uint32_t (2 * chunk_ent) * kTcK * 2; }
+constexpr int kTcFftWarps = 12;
+constexpr int kTcABufs = 2;                // the FFT of tile i + 1 fills one A buffer while the MMAs read tile i from the other
+// sync entries per B chunk -> N = 2 kTcChunkEnt columns (U and D column of every entry), chunk of N x 96 fp16 (18 KB): small
+// enough to leave room for twelve FFT warps AND two A buffers
+constexpr int kTcChunkEnt = 48;
+constexpr int kTcN = 2 * kTcChunkEnt;
+constexpr uint32_t kTcBBytes = uint32_t (kTcN) * kTcK * 2;
+constexpr size_t kTcSmemBytes = fft_smem_bytes (kTcFftWarps) + size_t (kTcABufs) * kTcABytes + kTcBBytes + 256;
+static_assert (kTcFftWarps % 4 == 0, "the MMA warpgroup has to start at a warp index divisible by four");
+static_assert (kTcN % kTcNB == 0, "a chunk is a whole number of wgmma blocks");
 
-template<int FFT_WARPS, int A_BUFS, int CHUNK_ENT> constexpr size_t
-tc_smem_bytes() { return fft_smem_bytes (FFT_WARPS) + size_t (A_BUFS) * kTcABytes + tc_b_bytes (CHUNK_ENT) + 256; }
-
-// host side: the 0/1 masks of all entries in operand layout, chunk after chunk ([ceil (n_ent / chunk_ent)][tc_b_bytes (chunk_ent)])
+// host side: the 0/1 masks of all entries in operand layout, chunk after chunk ([ceil (n_ent / kTcChunkEnt)][kTcBBytes])
 inline void
-tc_build_masks (const awm_sync_entry *ent, int n_ent, int chunk_ent, std::vector<unsigned char>& out)
+tc_build_masks (const awm_sync_entry *ent, int n_ent, std::vector<unsigned char>& out)
 {
-  const int n_chunks = (n_ent + chunk_ent - 1) / chunk_ent;
-  const size_t b_bytes = tc_b_bytes (chunk_ent);
-  out.assign (size_t (n_chunks) * b_bytes, 0);
+  const int n_chunks = (n_ent + kTcChunkEnt - 1) / kTcChunkEnt;
+  out.assign (size_t (n_chunks) * kTcBBytes, 0);
   const uint16_t one = 0x3c00;               // 1.0 in fp16
   for (int e = 0; e < n_ent; e++)
     {
-      unsigned char *chunk = out.data() + size_t (e / chunk_ent) * b_bytes;
-      const int col = 2 * (e % chunk_ent);
+      unsigned char *chunk = out.data() + size_t (e / kTcChunkEnt) * kTcBBytes;
+      const int col = 2 * (e % kTcChunkEnt);
       for (int i = 0; i < kUD; i++)
         {
-          memcpy (chunk + tc::operand_offset (2 * chunk_ent, col, ent[e].up[i]), &one, 2);
-          memcpy (chunk + tc::operand_offset (2 * chunk_ent, col + 1, ent[e].down[i]), &one, 2);
+          memcpy (chunk + tc::operand_offset (kTcN, col, ent[e].up[i]), &one, 2);
+          memcpy (chunk + tc::operand_offset (kTcN, col + 1, ent[e].down[i]), &one, 2);
         }
     }
 }
 
-template<int FFT_WARPS, int A_BUFS, int CHUNK_ENT> __global__ void __launch_bounds__ ((FFT_WARPS + kTcEpiWarps) * 32, 1)
+__global__ void __launch_bounds__ ((kTcFftWarps + kTcEpiWarps) * 32, 1)
 k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_out, int ld,
-                const unsigned char *__restrict__ masks /* [n_chunks][tc_b_bytes (CHUNK_ENT)] */, int n_ent, int n_chunks,
+                const unsigned char *__restrict__ masks /* [n_chunks][kTcBBytes] */, int n_ent, int n_chunks,
                 float2 *__restrict__ mags /* [4][n_ent][ld] */, unsigned char *__restrict__ have,
                 long long wav_first, long long wav_last, const float2 *g_tw, const float *g_win, int tma_ok /* stereo, pcm 16-byte aligned */)
 {
   using namespace tc;
-  constexpr int kTcN = 2 * CHUNK_ENT;
-  constexpr uint32_t kTcBBytes = tc_b_bytes (CHUNK_ENT);
-  static_assert (FFT_WARPS % 4 == 0, "the MMA warpgroup has to start at a warp index divisible by four");
-  static_assert (kTcN % kTcNB == 0, "a chunk is a whole number of wgmma blocks");
   extern __shared__ __align__ (16) unsigned char smem[];
-  FftSmem s = fft_smem_setup (smem, g_tw, g_win, FFT_WARPS);
+  FftSmem s = fft_smem_setup (smem, g_tw, g_win, kTcFftWarps);
   unsigned char *abuf = reinterpret_cast<unsigned char *> (s.extra);
-  unsigned char *bbuf = abuf + size_t (A_BUFS) * kTcABytes;
+  unsigned char *bbuf = abuf + size_t (kTcABufs) * kTcABytes;
   uint64_t *bars = reinterpret_cast<uint64_t *> (bbuf + kTcBBytes);
   uint64_t *a_full = bars, *a_empty = bars + 2, *b_full = bars + 4;
   uint64_t *pcm_bars = bars + 5;                                   // one per FFT warp: its next frame has landed in its transpose buffer
@@ -81,22 +80,22 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
     {
       for (int i = 0; i < 2; i++)
         {
-          mbar_init (&a_full[i], FFT_WARPS);
+          mbar_init (&a_full[i], kTcFftWarps);
           mbar_init (&a_empty[i], kTcEpiWarps);
         }
       mbar_init (b_full, 1);
-      for (int i = 0; i < FFT_WARPS; i++)
+      for (int i = 0; i < kTcFftWarps; i++)
         mbar_init (&pcm_bars[i], 1);
       fence_mbar_init();
     }
   // band columns 81 .. 95 of A are never written again and must be finite: clear everything once
-  for (uint32_t i = threadIdx.x; i < A_BUFS * kTcABytes / 16; i += blockDim.x)
+  for (uint32_t i = threadIdx.x; i < kTcABufs * kTcABytes / 16; i += blockDim.x)
     reinterpret_cast<uint4 *> (abuf)[i] = make_uint4 (0, 0, 0, 0);
   fence_proxy_async();
   __syncthreads();
   const int n_tiles = 4 * ((n_out + kTcTile - 1) / kTcTile);
 
-  if (w < FFT_WARPS)
+  if (w < kTcFftWarps)
     {
       // ===================================================================================== FFT warps
       // The PCM of a frame reaches the warp through the bulk-copy engine: while the second butterfly pass of frame i runs, the
@@ -118,7 +117,7 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
       auto by_tma = [&] (Frame fr) { return tma_ok && exists (fr) && wanted (fr) && frame_start (fr) + kFrame <= n_frames; };
       auto next_of = [&] (Frame fr)
         {
-          fr.r += FFT_WARPS;
+          fr.r += kTcFftWarps;
           if (fr.r >= kTcTile)
             {
               fr.r = w;
@@ -142,7 +141,7 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
       for (; exists (cur); it++)
         {
           const int shift_idx = cur.t & 3, f0 = (cur.t >> 2) * kTcTile;
-          const int a = it % A_BUFS, use = it / A_BUFS;
+          const int a = it % kTcABufs, use = it / kTcABufs;
           mbar_wait_relaxed (&a_empty[a], (use & 1) ^ 1);         // the MMAs that read this buffer last time are done
           unsigned char *A = abuf + size_t (a) * kTcABytes;
           const int t_now = cur.t;
@@ -218,7 +217,7 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
       // Per chunk: 2 (64-row halves) x kTcN / 32 (column blocks) x [2 (hi, lo) x 6 (K steps)] wgmma, each block written to `mags`
       // as soon as it is complete.  The mask chunk has one buffer: thread 0 loads the next chunk as soon as the whole warpgroup is
       // past the last MMA that reads the current one, and the load lands while the last blocks are stored.
-      const int wt = threadIdx.x - FFT_WARPS * 32, wi = wt >> 5;                  // thread / warp within the warpgroup
+      const int wt = threadIdx.x - kTcFftWarps * 32, wi = wt >> 5;                  // thread / warp within the warpgroup
       const uint32_t b_addr = smem_u32 (bbuf);
       auto load_b = [&] (int c)
         {
@@ -230,7 +229,7 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
       int it = 0, g = 0;
       for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, it++)
         {
-          const int a = it % A_BUFS, use = it / A_BUFS;
+          const int a = it % kTcABufs, use = it / kTcABufs;
           const int shift_idx = t & 3, f0 = (t >> 2) * kTcTile;
           const uint32_t a_addr = smem_u32 (abuf + size_t (a) * kTcABytes);
           mbar_wait_relaxed (&a_full[a], use & 1);                                // all FFT warps have delivered their rows of the tile
@@ -277,7 +276,7 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
                             load_b (0);
                         }
                     }
-                  const int e_base = c * CHUNK_ENT + nb * (kTcNB / 2) + (lane & 3);
+                  const int e_base = c * kTcChunkEnt + nb * (kTcNB / 2) + (lane & 3);
                   const int f = f0 + mh * 64 + wi * 16 + (lane >> 2);           // f + 8 < ld always (ld multiple of 128)
 #pragma unroll
                   for (int q = 0; q < kTcNB / 8; q++)

@@ -13,7 +13,6 @@
 #include "awm_approx_tc.cuh"
 #include "awm_embed_strip.cuh"
 #include "awm_embed_batch.cuh"
-#include "awm_viterbi_pair.cuh"
 
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -117,8 +116,8 @@ wall_now()
 struct SyncTab
 {
   DevBuf ent, off, sorted, groups;
-  DevBuf masks, masks48;              // 0/1 band masks of the entries as wgmma B operand chunks of 128 / 48 entries (awm_approx_tc.cuh)
-  int n_chunks = 0, n_chunks48 = 0;
+  DevBuf masks;                       // 0/1 band masks of the entries as wgmma B operand chunks of 48 entries (awm_approx_tc.cuh)
+  int n_chunks = 0;
   int n_groups = 0;
   int n_ent = 0, n_bits = 0, total_frames = 0;
   std::vector<awm_sync_entry> h_ent;
@@ -169,7 +168,7 @@ struct awm_ctx
   size_t n_scores_dev = 0;
   DevBuf cand_start, cand_noff, r_ud, r_cnt, rvalid, r_ent_ud, r_ent_flag, tw1024;   // refine
   DevBuf blk_start, D, raw;          // decode
-  DevBuf vit_raw, vit_off, vit_types, vit_delta, vit_dec, vit_bits, vit_err, vit_order;
+  DevBuf vit_raw, vit_off, vit_types, vit_delta, vit_dec, vit_bits, vit_err;
   DevBuf emb_in, emb_out, emb_in16, emb_out16, peaks, snr;
 
   PinArena pin;
@@ -365,7 +364,7 @@ awm_destroy (awm_ctx *ctx)
   cudaStreamSynchronize (ctx->stream);
   DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->have, &ctx->q, &ctx->scores, &ctx->a_ud, &ctx->a_cnt, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
                      &ctx->cand_start, &ctx->cand_noff, &ctx->r_ud, &ctx->r_cnt, &ctx->rvalid, &ctx->r_ent_ud, &ctx->r_ent_flag, &ctx->tw1024, &ctx->vit_off, &ctx->blk_start, &ctx->D, &ctx->raw,
-                     &ctx->vit_raw, &ctx->vit_types, &ctx->vit_delta, &ctx->vit_dec, &ctx->vit_bits, &ctx->vit_err, &ctx->vit_order,
+                     &ctx->vit_raw, &ctx->vit_types, &ctx->vit_delta, &ctx->vit_dec, &ctx->vit_bits, &ctx->vit_err,
                      &ctx->emb_in, &ctx->emb_out, &ctx->emb_in16, &ctx->emb_out16, &ctx->peaks, &ctx->snr, &ctx->rs_in, &ctx->rs_out, &ctx->rs_jobs, &ctx->pcm_rs,
                      &ctx->win512, &ctx->sp_clip, &ctx->sp_sub, &ctx->sp_mags, &ctx->sp_mag_jobs, &ctx->sp_cmp_jobs, &ctx->sp_best };
   for (DevBuf *b : bufs)
@@ -392,7 +391,6 @@ awm_destroy (awm_ctx *ctx)
         {
           s.ent.release();
           s.masks.release();
-          s.masks48.release();
           s.off.release();
           s.sorted.release();
           s.groups.release();
@@ -646,16 +644,12 @@ awm_set_sync_tables (awm_ctx *ctx, int key_slot, int mode, const awm_sync_entry 
   CK (cudaMemcpyAsync (t.groups.p, group_end.data(), group_end.size() * sizeof (int), cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaStreamSynchronize (ctx->stream));
   {
-    std::vector<unsigned char> masks, masks48;
-    tc_build_masks (entries, n_entries, 128, masks);
-    tc_build_masks (entries, n_entries, 48, masks48);
+    std::vector<unsigned char> masks;
+    tc_build_masks (entries, n_entries, masks);
     CK (t.masks.reserve (masks.size()));
-    CK (t.masks48.reserve (masks48.size()));
     CK (cudaMemcpyAsync (t.masks.p, masks.data(), masks.size(), cudaMemcpyHostToDevice, ctx->stream));
-    CK (cudaMemcpyAsync (t.masks48.p, masks48.data(), masks48.size(), cudaMemcpyHostToDevice, ctx->stream));
     CK (cudaStreamSynchronize (ctx->stream));
-    t.n_chunks = int (masks.size() / tc_b_bytes (128));
-    t.n_chunks48 = int (masks48.size() / tc_b_bytes (48));
+    t.n_chunks = int (masks.size() / kTcBBytes);
   }
   t.n_groups = int (group_end.size());
   t.n_ent = n_entries;
@@ -1028,9 +1022,8 @@ embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frame
   A.synth = ctx->synth.as<float>();
   const size_t smem = kEmbedSmem;
   if (set_smem (ctx, k_embed, smem)) return 1;
-  /* stereo audio in a 16-byte aligned buffer streams through k_embed_strip (awm_embed_strip.cuh); AWM_EMBED=tile keeps k_embed */
-  const char *env_embed = getenv ("AWM_EMBED");
-  const bool use_strip = channels == 2 && (reinterpret_cast<uintptr_t> (A.in) & 15) == 0 && !(env_embed && !strcmp (env_embed, "tile"));
+  /* stereo audio in a 16-byte aligned buffer streams through k_embed_strip (awm_embed_strip.cuh); anything else takes k_embed */
+  const bool use_strip = channels == 2 && (reinterpret_cast<uintptr_t> (A.in) & 15) == 0;
   if (use_strip)
     {
       if (!ctx->n_sms)
@@ -1438,42 +1431,27 @@ awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
   CK (ctx->a_cnt.reserve (size_t (n_starts) * 4 * t.n_bits * sizeof (int)));
   CK (ctx->scores.reserve (size_t (n_starts) * 4 * sizeof (awm_search_score)));
   const double norm_div = water_delta < 0.080 ? water_delta : 0.080;     // normalize_sync_quality, src/syncfinder.cc:90
-  /* default: per-frame entry sums + one streaming gather (awm_approx_mags.cuh); AWM_APPROX=ring selects the kernel that walks
-   * the dB matrix per start frame in the reference's exact summation order */
-  static const bool force_ring = [] { const char *e = getenv ("AWM_APPROX"); return e && !strcmp (e, "ring"); } ();
+  /* default: entry sums on the tensor cores (k_stft_mags_tc, awm_approx_tc.cuh) + one streaming gather.  AWM_APPROX selects the
+   * test references: simt = the same entry sums on the fp32 pipes (k_stft_mags, awm_approx_mags.cuh); ring = the kernel that walks
+   * the dB matrix per start frame in the reference's exact summation order.  Read per call: tests compare the kernels in one process */
+  const char *env_approx = getenv ("AWM_APPROX");
+  const bool force_ring = env_approx && !strcmp (env_approx, "ring"), force_simt = env_approx && !strcmp (env_approx, "simt");
   if (!force_ring && t.n_ent <= kGatherMaxEntries)
     {
       CK (ctx->a_mags.reserve (size_t (4) * t.n_ent * ld * sizeof (float2)));
-      /* entry sums on the tensor cores (k_stft_mags_tc); AWM_APPROX=simt keeps them on the fp32 pipes (k_stft_mags).  Variants
-       * (AWM_TC): default 12x2 = twelve FFT warps, two A buffers, mask chunks of 48 entries; 8x2 = eight FFT warps, chunks of 128
-       * entries; 12x1 = twelve FFT warps, one A buffer, chunks of 128 */
-      const char *env_approx = getenv ("AWM_APPROX"), *env_tc = getenv ("AWM_TC");       // read per call: tests compare the variants in one process
-      const bool force_simt = env_approx && !strcmp (env_approx, "simt");
-      const bool tc_12x1 = env_tc && !strcmp (env_tc, "12x1"), tc_8x2 = env_tc && !strcmp (env_tc, "8x2");
       if (!force_simt)
         {
           if (!ctx->n_sms)
             CK (cudaDeviceGetAttribute (&ctx->n_sms, cudaDevAttrMultiProcessorCount, ctx->device));
           const int n_tiles = 4 * int ((n_out + kTcTile - 1) / kTcTile);
           const unsigned grid = unsigned (std::min (n_tiles, ctx->n_sms));
-          const char *env_tma = getenv ("AWM_TC_PCM");                      // AWM_TC_PCM=ldg: frames by global loads instead of bulk copies
-          const int tma_ok = ctx->pcm_ch == 2 && (reinterpret_cast<uintptr_t> (ctx->pcm) & 15) == 0 && !(env_tma && !strcmp (env_tma, "ldg"));
-#define AWM_LAUNCH_TC(FW, AB, CE, MASKS, NCH)                                                                                              \
-          {                                                                                                                                 \
-            const size_t smem = tc_smem_bytes<FW, AB, CE>();                                                                                \
-            if (set_smem (ctx, k_stft_mags_tc<FW, AB, CE>, smem)) return 1;                                                                 \
-            PROF (ctx);                                                                                                                     \
-            k_stft_mags_tc<FW, AB, CE><<<grid, (FW + kTcEpiWarps) * 32, smem, ctx->stream>>> (ctx->pcm, (long long) ctx->pcm_frames,    \
-              ctx->pcm_ch, int (n_out), ld, MASKS.as<unsigned char>(), t.n_ent, NCH, ctx->a_mags.as<float2>(),                              \
-              ctx->have.as<unsigned char>(), (long long) wav_first, (long long) wav_last, ctx->tw.as<float2>(), ctx->win.as<float>(), tma_ok); \
-          }
-          if (tc_12x1)
-            AWM_LAUNCH_TC (12, 1, 128, t.masks, t.n_chunks)
-          else if (tc_8x2)
-            AWM_LAUNCH_TC (8, 2, 128, t.masks, t.n_chunks)
-          else
-            AWM_LAUNCH_TC (12, 2, 48, t.masks48, t.n_chunks48)
-#undef AWM_LAUNCH_TC
+          /* stereo PCM in a 16-byte aligned buffer reaches the FFT warps by bulk copies, anything else by global loads */
+          const int tma_ok = ctx->pcm_ch == 2 && (reinterpret_cast<uintptr_t> (ctx->pcm) & 15) == 0;
+          if (set_smem (ctx, k_stft_mags_tc, kTcSmemBytes)) return 1;
+          PROF (ctx);
+          k_stft_mags_tc<<<grid, (kTcFftWarps + kTcEpiWarps) * 32, kTcSmemBytes, ctx->stream>>> (ctx->pcm, (long long) ctx->pcm_frames,
+            ctx->pcm_ch, int (n_out), ld, t.masks.as<unsigned char>(), t.n_ent, t.n_chunks, ctx->a_mags.as<float2>(),
+            ctx->have.as<unsigned char>(), (long long) wav_first, (long long) wav_last, ctx->tw.as<float2>(), ctx->win.as<float>(), tma_ok);
           LAUNCH_CHECK ("k_stft_mags_tc");
           prof_bytes (ctx, double (ctx->pcm_frames) * ctx->pcm_ch * sizeof (float) + double (4) * t.n_ent * n_out * sizeof (float2));   /* PCM in, entry sums out */
         }
@@ -2150,14 +2128,10 @@ awm_viterbi (awm_ctx *ctx, const float *raw_bits, size_t n_jobs, int n_msg_bits,
     }
   CK (cudaSetDevice (ctx->device));
   const size_t max_jobs = 512;
-  /* default: one CTA per code word (k_viterbi).  AWM_VITERBI=pair: a cluster of two CTAs per word with the metrics exchanged through
-   * distributed shared memory (k_viterbi_pair, awm_viterbi_pair.cuh) -- same bits; every trellis step pays a cluster-wide barrier */
-  const char *env_vit = getenv ("AWM_VITERBI");
-  const bool use_pair = env_vit && !strcmp (env_vit, "pair");
-  const size_t smem = use_pair ? viterbi_pair_smem_bytes (steps) : viterbi_smem_bytes (steps);
+  const size_t smem = viterbi_smem_bytes (steps);
   if (smem > 220 * 1024)
     return fail (ctx, "awm_viterbi: %d message bits are more than the kernel holds in shared memory", n_msg_bits);
-  if (use_pair ? set_smem (ctx, k_viterbi_pair, smem) : set_smem (ctx, k_viterbi, smem)) return 1;
+  if (set_smem (ctx, k_viterbi, smem)) return 1;
   for (size_t j0 = 0; j0 < n_jobs; j0 += max_jobs)
     {
       const size_t nj = std::min (max_jobs, n_jobs - j0);
@@ -2171,7 +2145,6 @@ awm_viterbi (awm_ctx *ctx, const float *raw_bits, size_t n_jobs, int n_msg_bits,
       CK (ctx->vit_dec.reserve (nj * steps * kVitWords * sizeof (uint32_t)));
       CK (ctx->vit_bits.reserve (nj * n_msg_bits));
       CK (ctx->vit_err.reserve (nj * sizeof (float)));
-      CK (ctx->vit_order.reserve (nj * sizeof (int)));
       /* host inputs / outputs pass through page-locked staging: the three uploads, the launch and the two downloads queue up
        * without the host waiting in between */
       ctx->pin.reset();
@@ -2179,38 +2152,21 @@ awm_viterbi (awm_ctx *ctx, const float *raw_bits, size_t n_jobs, int n_msg_bits,
       float *h_in = raw_on_device ? nullptr : ctx->pin.get<float> (size_t (n_raw));
       long long *h_rel = ctx->pin.get<long long> (nj);
       int *h_types = ctx->pin.get<int> (nj);
-      int *h_order = ctx->pin.get<int> (nj);
       unsigned char *h_bits = ctx->pin.get<unsigned char> (nj * n_msg_bits);
       float *h_err = ctx->pin.get<float> (nj);
-      if ((!raw_on_device && !h_in) || !h_rel || !h_types || !h_order || !h_bits || !h_err)
+      if ((!raw_on_device && !h_in) || !h_rel || !h_types || !h_bits || !h_err)
         return fail (ctx, "awm_viterbi: out of page-locked memory");
       if (h_in)
         memcpy (h_in, raw_bits + base, size_t (n_raw) * sizeof (float));
       std::copy (rel.begin(), rel.end(), h_rel);
       std::copy (block_types + j0, block_types + j0 + nj, h_types);
-      {
-        /* AB words (twice the adds of an A or B word) go first in the grid, the shorter words fill the SMs they free */
-        size_t k = 0;
-        for (size_t j = 0; j < nj; j++)
-          if (h_types[j] == AWM_BLOCK_AB)
-            h_order[k++] = int (j);
-        for (size_t j = 0; j < nj; j++)
-          if (h_types[j] != AWM_BLOCK_AB)
-            h_order[k++] = int (j);
-      }
       CK (cudaMemcpyAsync (ctx->vit_raw.p, h_in ? h_in : raw_bits + base, n_raw * sizeof (float), cudaMemcpyDefault, ctx->stream));
       CK (cudaMemcpyAsync (ctx->vit_off.p, h_rel, nj * sizeof (long long), cudaMemcpyHostToDevice, ctx->stream));
       CK (cudaMemcpyAsync (ctx->vit_types.p, h_types, nj * sizeof (int), cudaMemcpyHostToDevice, ctx->stream));
-      CK (cudaMemcpyAsync (ctx->vit_order.p, h_order, nj * sizeof (int), cudaMemcpyHostToDevice, ctx->stream));
       PROF (ctx);
-      if (use_pair)
-        k_viterbi_pair<<<unsigned (2 * nj), kVitThreads, smem, ctx->stream>>> (ctx->vit_raw.as<float>(), ctx->vit_off.as<long long>(), n_msg_bits, ctx->vit_types.as<int>(),
-                                                                         hard, steps, ctx->vit_order.as<int>(), ctx->vit_dec.as<uint32_t>(),
-                                                                         ctx->vit_bits.as<unsigned char>(), ctx->vit_err.as<float>());
-      else
-        k_viterbi<<<unsigned (nj), kVitThreads, smem, ctx->stream>>> (ctx->vit_raw.as<float>(), ctx->vit_off.as<long long>(), n_msg_bits, ctx->vit_types.as<int>(), hard,
-                                                                    steps, ctx->vit_dec.as<uint32_t>(),
-                                                                    ctx->vit_bits.as<unsigned char>(), ctx->vit_err.as<float>());
+      k_viterbi<<<unsigned (nj), kVitThreads, smem, ctx->stream>>> (ctx->vit_raw.as<float>(), ctx->vit_off.as<long long>(), n_msg_bits, ctx->vit_types.as<int>(), hard,
+                                                                  steps, ctx->vit_dec.as<uint32_t>(),
+                                                                  ctx->vit_bits.as<unsigned char>(), ctx->vit_err.as<float>());
       LAUNCH_CHECK ("k_viterbi");
       CK (cudaMemcpyAsync (h_bits, ctx->vit_bits.p, nj * n_msg_bits, cudaMemcpyDeviceToHost, ctx->stream));
       CK (cudaMemcpyAsync (h_err, ctx->vit_err.p, nj * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));

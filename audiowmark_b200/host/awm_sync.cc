@@ -298,7 +298,7 @@ SyncFinder::search (const vector<Key>& key_list, size_t n_frames, int n_channels
           size_t n_scores = 0;
           ok = awm_sync_approx (ctx, slot, amode, wav_first, wav_last, Params::water_delta, nullptr, 0, &n_scores) == 0;
           /* the scores stay on the device; normally only the peaks that matter come back */
-          gpu_selected = ok && n_scores && !getenv ("AWM_HOST_SELECT") && select_candidates_gpu (ctx, Params::sync_threshold2 * 0.75, scores);
+          gpu_selected = ok && n_scores && select_candidates_gpu (ctx, Params::sync_threshold2 * 0.75, scores);
           if (gpu_selected)
             n_scores = 0;                         // nothing else to fetch
           if (ok && n_scores > all_cap)
