@@ -31,7 +31,7 @@ EXPORTS = [
     "awm_fft_r2c", "awm_fft_c2r", "awm_set_embed_tables", "awm_set_sync_tables", "awm_set_mix_tables",
     "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_decode_blocks", "awm_viterbi",
     "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_is_device_pointer", "awm_speed_scan", "awm_embed_resampled", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_prefetch_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
-    "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch",
+    "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch", "awm_batch_rates_validate", "awm_embed_batch_rates",
 ]
 
 _lib = None
@@ -70,6 +70,18 @@ def batch_validate(items, n_values: int) -> str:
     it = np.array([tuple(int(v) for v in t) for t in items], BATCH_ITEM)
     err = ctypes.create_string_buffer(256)
     rc = load().awm_batch_validate(_ptr(it), ctypes.c_size_t(len(it)), ctypes.c_size_t(n_values), err, ctypes.c_size_t(len(err)))
+    return err.value.decode() if rc else ""
+
+
+def batch_rates_validate(items, n_values: int, sample_rates, n_emit=None, mark_sample_rate: int = 44100) -> str:
+    """awm_batch_rates_validate: '' if the items fit a packed buffer of n_values values and every rate (and n_emit, if given) is
+    acceptable, else the reason"""
+    it = np.array([tuple(int(v) for v in t) for t in items], BATCH_ITEM)
+    rates = np.ascontiguousarray(sample_rates, np.int32)
+    emit = None if n_emit is None else np.ascontiguousarray(n_emit, np.uint64)
+    err = ctypes.create_string_buffer(256)
+    rc = load().awm_batch_rates_validate(_ptr(it), ctypes.c_size_t(len(it)), ctypes.c_size_t(n_values), _ptr(rates), _ptr(emit),
+                                         ctypes.c_int(mark_sample_rate), err, ctypes.c_size_t(len(err)))
     return err.value.decode() if rc else ""
 
 

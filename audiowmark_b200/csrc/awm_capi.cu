@@ -13,6 +13,7 @@
 #include "awm_approx_tc.cuh"
 #include "awm_embed_strip.cuh"
 #include "awm_embed_batch.cuh"
+#include "awm_batch_rates.cuh"
 
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -149,6 +150,7 @@ struct awm_ctx
   DevBuf frame_mod; int embed_fpb = 0;
   DevBuf roles; int roles_fpb = 0, roles_n_coded = 0;         // batched embed: role table of one key
   DevBuf batch_items, batch_coded;
+  DevBuf rate_items, rate_scratch;                           // batched embed at other sample rates: work list, per-wave scratch
   KeyTab keys[AWM_MAX_KEYS];
 
   // bound PCM
@@ -362,7 +364,7 @@ awm_destroy (awm_ctx *ctx)
     return;
   cudaSetDevice (ctx->device);
   cudaStreamSynchronize (ctx->stream);
-  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->have, &ctx->q, &ctx->scores, &ctx->a_ud, &ctx->a_cnt, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
+  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->rate_items, &ctx->rate_scratch, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->have, &ctx->q, &ctx->scores, &ctx->a_ud, &ctx->a_cnt, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
                      &ctx->cand_start, &ctx->cand_noff, &ctx->r_ud, &ctx->r_cnt, &ctx->rvalid, &ctx->r_ent_ud, &ctx->r_ent_flag, &ctx->tw1024, &ctx->vit_off, &ctx->blk_start, &ctx->D, &ctx->raw,
                      &ctx->vit_raw, &ctx->vit_types, &ctx->vit_delta, &ctx->vit_dec, &ctx->vit_bits, &ctx->vit_err,
                      &ctx->emb_in, &ctx->emb_out, &ctx->emb_in16, &ctx->emb_out16, &ctx->peaks, &ctx->snr, &ctx->rs_in, &ctx->rs_out, &ctx->rs_jobs, &ctx->pcm_rs,
@@ -1255,6 +1257,132 @@ awm_batch_validate (const awm_batch_item *items, size_t n_items, size_t n_values
   return 0;
 }
 
+namespace {
+
+/* float images of a packed batch buffer: the caller's own buffers where they are float device memory, else the context's staging
+ * buffers, which receive the input (16 bit input converted on the device) */
+int
+batch_images (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_values, const float **d_in_out, float **d_out_out)
+{
+  const bool in_dev = is_device_ptr (in_v), out_dev = is_device_ptr (out_v);
+  const float *d_in = !s16 && in_dev ? static_cast<const float *> (in_v) : nullptr;
+  float *d_out = !s16 && out_dev ? static_cast<float *> (out_v) : nullptr;
+  if (!d_in)
+    {
+      CK (ctx->emb_in.reserve (n_values * sizeof (float)));
+      d_in = ctx->emb_in.as<float>();
+    }
+  if (!d_out)
+    {
+      CK (ctx->emb_out.reserve (n_values * sizeof (float)));
+      d_out = ctx->emb_out.as<float>();
+    }
+  if (s16)
+    {
+      const int16_t *d_in16 = static_cast<const int16_t *> (in_v);
+      if (!in_dev)
+        {
+          CK (ctx->emb_in16.reserve (n_values * sizeof (int16_t)));
+          CK (cudaMemcpyAsync (ctx->emb_in16.p, in_v, n_values * sizeof (int16_t), cudaMemcpyHostToDevice, ctx->stream));
+          d_in16 = ctx->emb_in16.as<int16_t>();
+        }
+      PROF (ctx);
+      k_s16_to_f32<<<unsigned (((n_values + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (d_in16, ctx->emb_in.as<float>(), (long long) n_values);
+      LAUNCH_CHECK ("k_s16_to_f32");
+    }
+  else if (!in_dev)
+    CK (cudaMemcpyAsync (ctx->emb_in.p, in_v, n_values * sizeof (float), cudaMemcpyHostToDevice, ctx->stream));
+  *d_in_out = d_in;
+  *d_out_out = d_out;
+  return 0;
+}
+
+/* the float image d_out of batch_images into out_v (16 bit output converted on the device), the --snr sums into snr_power */
+int
+batch_finish (awm_ctx *ctx, void *out_v, bool s16, size_t n_values, const float *d_out, double *snr_power, size_t n_snr)
+{
+  const bool out_dev = is_device_ptr (out_v);
+  if (s16)
+    {
+      int16_t *d_out16 = static_cast<int16_t *> (out_v);
+      if (!out_dev)
+        {
+          CK (ctx->emb_out16.reserve (n_values * sizeof (int16_t)));
+          d_out16 = ctx->emb_out16.as<int16_t>();
+        }
+      PROF (ctx);
+      k_f32_to_s16<<<unsigned (((n_values + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (d_out, d_out16, (long long) n_values);
+      LAUNCH_CHECK ("k_f32_to_s16");
+      if (!out_dev)
+        CK (cudaMemcpyAsync (out_v, d_out16, n_values * sizeof (int16_t), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+  else if (!out_dev)
+    CK (cudaMemcpyAsync (out_v, d_out, n_values * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
+  if (snr_power && n_snr)
+    CK (cudaMemcpyAsync (snr_power, ctx->snr.p, 2 * n_snr * sizeof (double), cudaMemcpyDeviceToHost, ctx->stream));
+  if (!out_dev || snr_power)
+    CK (cudaStreamSynchronize (ctx->stream));
+  return 0;
+}
+
+/* k_embed_batch work list entry of a non-empty item with awm_embed's geometry (limiter_block 0: no block peaks); advances the
+ * launch's tile / limiter CTA counters and the flat peak array */
+BatchItem
+batch_entry (long long v0, long long n_frames, int C, int item, int limiter_block, long long& n_tiles, long long& n_lim, long long& n_peaks)
+{
+  BatchItem b;
+  b.v0 = v0;
+  b.n_frames = n_frames;
+  b.C = C;
+  b.item = item;
+  const long long n_proc = (b.n_frames + kFrame - 1) / kFrame + 1;
+  b.tile0 = n_tiles;
+  b.lim0 = n_lim;
+  b.peak0 = n_peaks;
+  b.n_blocks = limiter_block > 0 ? (n_proc * kFrame + limiter_block - 1) / limiter_block + 2 : 0;   // as awm_embed's
+  n_tiles += (n_proc + kEmbedTile - 1) / kEmbedTile;
+  n_lim += (b.n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter);
+  n_peaks += b.n_blocks;
+  return b;
+}
+
+/* k_embed_batch over the n_list items at d_items (v0 relative to in / out), then k_limiter_batch when limiter_block > 0.
+ * Peaks go to ctx->peaks (zeroed by the caller), --snr sums to d_snr (null: none); delta_only: write the watermark signal alone */
+int
+launch_embed_batch (awm_ctx *ctx, const float *in, float *out, const BatchItem *d_items, int n_list, long long n_tiles, long long n_lim,
+                    int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling, double *d_snr, int delta_only)
+{
+  EmbedArgs A = {};
+  A.in = in;
+  A.out = out;
+  A.fpb = ctx->roles_fpb;
+  A.frame_number0 = 2LL * A.fpb - frames_pad_start;       // first_frame_number 0: every item is a stream of its own
+  A.pow_up = 0.5f * float (-water_delta * 1);
+  A.pow_down = 0.5f * float (-water_delta * -1);
+  A.limiter_block = limiter_block;
+  A.peaks = ctx->peaks.as<unsigned>();
+  A.snr = d_snr;
+  A.snr_pos1 = LLONG_MAX;
+  A.delta_only = delta_only;
+  A.tw = ctx->tw.as<float2>();
+  A.win = ctx->win.as<float>();
+  A.synth = ctx->synth.as<float>();
+  if (set_smem (ctx, k_embed_batch, kEmbedBatchSmem)) return 1;
+  PROF (ctx);
+  k_embed_batch<<<unsigned (n_tiles), kEmbedWarps * 32, kEmbedBatchSmem, ctx->stream>>> (A, d_items, n_list, ctx->roles.as<uint16_t>(),
+                                                                                        ctx->batch_coded.as<uint8_t>(), ctx->roles_n_coded);
+  LAUNCH_CHECK ("k_embed_batch");
+  if (limiter_block > 0)
+    {
+      PROF (ctx);
+      k_limiter_batch<<<unsigned (n_lim), 256, 0, ctx->stream>>> (out, d_items, n_list, limiter_block, limiter_ceiling, ctx->peaks.as<unsigned>());
+      LAUNCH_CHECK ("k_limiter_batch");
+    }
+  return 0;
+}
+
+} // namespace
+
 int
 awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
                  const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
@@ -1273,36 +1401,10 @@ awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t
     return 0;
   CK (cudaSetDevice (ctx->device));
   const bool s16 = is_s16 != 0;
-  const bool in_dev = is_device_ptr (in_v), out_dev = is_device_ptr (out_v);
-  /* float images of in / out: the caller's own buffers where they are float device memory, else the context's staging buffers */
-  const float *d_in = !s16 && in_dev ? static_cast<const float *> (in_v) : nullptr;
-  float *d_out = !s16 && out_dev ? static_cast<float *> (out_v) : nullptr;
-  if (!d_in)
-    {
-      CK (ctx->emb_in.reserve (n_values * sizeof (float)));
-      d_in = ctx->emb_in.as<float>();
-    }
-  if (!d_out)
-    {
-      CK (ctx->emb_out.reserve (n_values * sizeof (float)));
-      d_out = ctx->emb_out.as<float>();
-    }
-  const unsigned conv_grid = unsigned (((n_values + 1) / 2 + 255) / 256);
-  if (s16)
-    {
-      const int16_t *d_in16 = static_cast<const int16_t *> (in_v);
-      if (!in_dev)
-        {
-          CK (ctx->emb_in16.reserve (n_values * sizeof (int16_t)));
-          CK (cudaMemcpyAsync (ctx->emb_in16.p, in_v, n_values * sizeof (int16_t), cudaMemcpyHostToDevice, ctx->stream));
-          d_in16 = ctx->emb_in16.as<int16_t>();
-        }
-      PROF (ctx);
-      k_s16_to_f32<<<conv_grid, 256, 0, ctx->stream>>> (d_in16, ctx->emb_in.as<float>(), (long long) n_values);
-      LAUNCH_CHECK ("k_s16_to_f32");
-    }
-  else if (!in_dev)
-    CK (cudaMemcpyAsync (ctx->emb_in.p, in_v, n_values * sizeof (float), cudaMemcpyHostToDevice, ctx->stream));
+  const float *d_in;
+  float *d_out;
+  if (batch_images (ctx, in_v, out_v, s16, n_values, &d_in, &d_out))
+    return 1;
 
   /* work list: non-empty items with their first tile, first limiter CTA and block peaks */
   std::vector<BatchItem> list;
@@ -1311,22 +1413,9 @@ awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t
   for (size_t i = 0; i < n_items; i++)
     {
       covered += items[i].n_frames * uint64_t (items[i].channels);
-      if (!items[i].n_frames)
-        continue;
-      BatchItem b;
-      b.v0 = (long long) items[i].value_offset;
-      b.n_frames = (long long) items[i].n_frames;
-      b.C = items[i].channels;
-      b.item = int (i);
-      const long long n_proc = (b.n_frames + kFrame - 1) / kFrame + 1;
-      b.tile0 = n_tiles;
-      b.lim0 = n_lim;
-      b.peak0 = n_peaks;
-      b.n_blocks = limiter_block > 0 ? (n_proc * kFrame + limiter_block - 1) / limiter_block + 2 : 0;   // as awm_embed's
-      n_tiles += (n_proc + kEmbedTile - 1) / kEmbedTile;
-      n_lim += (b.n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter);
-      n_peaks += b.n_blocks;
-      list.push_back (b);
+      if (items[i].n_frames)
+        list.push_back (batch_entry ((long long) items[i].value_offset, (long long) items[i].n_frames, items[i].channels, int (i), limiter_block,
+                                     n_tiles, n_lim, n_peaks));
     }
   if (n_tiles >= INT_MAX || list.size() >= size_t (INT_MAX))
     return fail (ctx, "awm_embed_batch: batch too large (%lld tiles)", n_tiles);
@@ -1349,54 +1438,11 @@ awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t
           CK (ctx->snr.reserve (2 * n_items * sizeof (double)));
           CK (cudaMemsetAsync (ctx->snr.p, 0, 2 * n_items * sizeof (double), ctx->stream));
         }
-      EmbedArgs A = {};
-      A.in = d_in;
-      A.out = d_out;
-      A.fpb = ctx->roles_fpb;
-      A.frame_number0 = 2LL * A.fpb - frames_pad_start;       // first_frame_number 0: every item is a stream of its own
-      A.pow_up = 0.5f * float (-water_delta * 1);
-      A.pow_down = 0.5f * float (-water_delta * -1);
-      A.limiter_block = limiter_block;
-      A.peaks = ctx->peaks.as<unsigned>();
-      A.snr = snr_power ? ctx->snr.as<double>() : nullptr;
-      A.snr_pos1 = LLONG_MAX;
-      A.tw = ctx->tw.as<float2>();
-      A.win = ctx->win.as<float>();
-      A.synth = ctx->synth.as<float>();
-      const BatchItem *d_items = ctx->batch_items.as<BatchItem>();
-      if (set_smem (ctx, k_embed_batch, kEmbedBatchSmem)) return 1;
-      PROF (ctx);
-      k_embed_batch<<<unsigned (n_tiles), kEmbedWarps * 32, kEmbedBatchSmem, ctx->stream>>> (A, d_items, int (list.size()), ctx->roles.as<uint16_t>(),
-                                                                                            ctx->batch_coded.as<uint8_t>(), ctx->roles_n_coded);
-      LAUNCH_CHECK ("k_embed_batch");
-      if (limiter_block > 0)
-        {
-          PROF (ctx);
-          k_limiter_batch<<<unsigned (n_lim), 256, 0, ctx->stream>>> (d_out, d_items, int (list.size()), limiter_block, limiter_ceiling, ctx->peaks.as<unsigned>());
-          LAUNCH_CHECK ("k_limiter_batch");
-        }
+      if (launch_embed_batch (ctx, d_in, d_out, ctx->batch_items.as<BatchItem>(), int (list.size()), n_tiles, n_lim, frames_pad_start, water_delta,
+                              limiter_block, limiter_ceiling, snr_power ? ctx->snr.as<double>() : nullptr, 0))
+        return 1;
     }
-  if (s16)
-    {
-      int16_t *d_out16 = static_cast<int16_t *> (out_v);
-      if (!out_dev)
-        {
-          CK (ctx->emb_out16.reserve (n_values * sizeof (int16_t)));
-          d_out16 = ctx->emb_out16.as<int16_t>();
-        }
-      PROF (ctx);
-      k_f32_to_s16<<<conv_grid, 256, 0, ctx->stream>>> (d_out, d_out16, (long long) n_values);
-      LAUNCH_CHECK ("k_f32_to_s16");
-      if (!out_dev)
-        CK (cudaMemcpyAsync (out_v, d_out16, n_values * sizeof (int16_t), cudaMemcpyDeviceToHost, ctx->stream));
-    }
-  else if (!out_dev)
-    CK (cudaMemcpyAsync (out_v, d_out, n_values * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
-  if (snr_power && !list.empty())
-    CK (cudaMemcpyAsync (snr_power, ctx->snr.p, 2 * n_items * sizeof (double), cudaMemcpyDeviceToHost, ctx->stream));
-  if (!out_dev || snr_power)
-    CK (cudaStreamSynchronize (ctx->stream));
-  return 0;
+  return batch_finish (ctx, out_v, s16, n_values, d_out, snr_power, list.empty() ? 0 : n_items);
 }
 
 /* ---------------------------------------------------------------- sync search */
@@ -2206,22 +2252,39 @@ rs_window (double x)        /* three-term cosine window on [-1, 1] */
 /* filter table for one conversion ratio: g(d) = fc sinc (fc d) w (d / h), fc = min (1, ratio), h = ceil (hlen / fc) input
  * frames to each side; row p holds the 2h taps for a fractional position of p / 256.  Built on the host in double (a
  * few ms, cached per ratio) so that every implementation that evaluates the same formula has the same float table. */
+constexpr size_t kCoefCacheCap = 1024;
+
+/* room for n_new filter tables: the cache is emptied when it would grow past kCoefCacheCap (data dependent ratios accumulate in
+ * long running hosts) */
+int
+coef_cache_room (awm_ctx *ctx, size_t n_new)
+{
+  if (ctx->coef_cache.size() + n_new <= kCoefCacheCap)
+    return 0;
+  CK (cudaStreamSynchronize (ctx->stream));
+  for (auto& ct : ctx->coef_cache)
+    ct.second.buf.release();
+  ctx->coef_cache.clear();
+  return 0;
+}
+
+bool
+resample_ratio_ok (double ratio)
+{
+  return ratio > 1.0 / 64 && ratio < 64;
+}
+
 int
 coef_table (awm_ctx *ctx, double ratio, int hlen, const float **coef, int *h_out)
 {
-  if (!(ratio > 1.0 / 64 && ratio < 64) || hlen < 8 || hlen > 96)
+  if (!resample_ratio_ok (ratio) || hlen < 8 || hlen > 96)
     return fail (ctx, "resampler: ratio %g / hlen %d not supported", ratio, hlen);
   auto key = std::make_pair (ratio, hlen);
   auto it = ctx->coef_cache.find (key);
   if (it == ctx->coef_cache.end())
     {
-      if (ctx->coef_cache.size() >= 1024)          /* data dependent ratios accumulate in long running hosts */
-        {
-          CK (cudaStreamSynchronize (ctx->stream));
-          for (auto& ct : ctx->coef_cache)
-            ct.second.buf.release();
-          ctx->coef_cache.clear();
-        }
+      if (coef_cache_room (ctx, 1))
+        return 1;
       const double fc = ratio < 1 ? ratio : 1;
       const int h = int (ceil (hlen / fc));
       const int taps = 2 * h, rows = kResamplePhases + 1;
@@ -2250,6 +2313,15 @@ coef_table (awm_ctx *ctx, double ratio, int hlen, const float **coef, int *h_out
   *coef = it->second.buf.as<float>();
   *h_out = it->second.h;
   return 0;
+}
+
+/* frames at the watermark rate an item of awm_embed_resampled needs: up to the highest tap of output n_emit - 1 (> 0), in whole
+ * 1024-frames */
+long long
+resampled_n44 (uint64_t n_emit, double step_out, int h_out)
+{
+  const long long top = (long long) floor (double (n_emit - 1) * step_out) + h_out;
+  return (top / kFrame + 1) * kFrame;
 }
 
 int
@@ -2423,9 +2495,7 @@ awm_embed_resampled (awm_ctx *ctx, const float *in, float *out, size_t n_frames,
     return 1;
   /* watermark frames needed for the emitted output: highest tap of output n_emit - 1 */
   const double step_out = 1.0 / r_out;
-  const long long top = (long long) floor (double (n_emit - 1) * step_out) + h_out;
-  const long long n_blocks44 = top / kFrame + 1;
-  const long long n44 = n_blocks44 * kFrame;
+  const long long n44 = resampled_n44 (n_emit, step_out, h_out), n_blocks44 = n44 / kFrame;
   const size_t n_val = n_frames * channels;
   const bool in_dev = is_device_ptr (in), out_dev = is_device_ptr (out);
   const float *d_in = in;
@@ -2522,6 +2592,224 @@ awm_embed_resampled (awm_ctx *ctx, const float *in, float *out, size_t n_frames,
   if (!out_dev || snr_power)
     CK (cudaStreamSynchronize (ctx->stream));
   return 0;
+}
+
+/* ---------------------------------------------------------------- batched embed at any sample rate */
+
+namespace {
+
+constexpr size_t kBatchMaxRates = 256;                          // different resampled rates per call: two filter tables each
+constexpr size_t kBatchDefaultScratch = size_t (4) << 30;       // per-wave scratch when the caller passes 0
+
+} // namespace
+
+int
+awm_batch_rates_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const int *sample_rates, const uint64_t *n_emit,
+                          int mark_sample_rate, char *err, size_t err_cap)
+{
+  if (awm_batch_validate (items, n_items, n_values, err, err_cap))
+    return 1;
+  char why[200] = "";
+  std::vector<int> rates;
+  if (mark_sample_rate <= 0)
+    snprintf (why, sizeof (why), "mark sample rate %d must be > 0", mark_sample_rate);
+  else if (n_items && !sample_rates)
+    snprintf (why, sizeof (why), "sample rate list is NULL");
+  for (size_t i = 0; i < n_items && !why[0]; i++)
+    {
+      const int r = sample_rates[i];
+      if (r <= 0)
+        snprintf (why, sizeof (why), "batch item %zu: sample rate %d must be > 0", i, r);
+      else if (r == mark_sample_rate)
+        continue;
+      else if (!resample_ratio_ok (double (mark_sample_rate) / r) || !resample_ratio_ok (double (r) / mark_sample_rate))
+        snprintf (why, sizeof (why), "batch item %zu: sample rate %d is outside the resampler's range (%d Hz / 64 .. %d Hz * 64, exclusive)",
+                  i, r, mark_sample_rate, mark_sample_rate);
+      else if (n_emit && n_emit[i] < items[i].n_frames)
+        snprintf (why, sizeof (why), "batch item %zu: n_emit %llu is less than n_frames %llu", i, (unsigned long long) n_emit[i],
+                  (unsigned long long) items[i].n_frames);
+      else
+        rates.push_back (r);
+    }
+  std::sort (rates.begin(), rates.end());
+  rates.erase (std::unique (rates.begin(), rates.end()), rates.end());
+  if (!why[0] && rates.size() > kBatchMaxRates)
+    snprintf (why, sizeof (why), "%zu different sample rates (at most %zu per call)", rates.size(), kBatchMaxRates);
+  if (err && err_cap)
+    snprintf (err, err_cap, "%s", why);
+  return why[0] ? 1 : 0;
+}
+
+int
+awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                       const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate, int frames_pad_start,
+                       double water_delta, int limiter_ms, float limiter_ceiling, double *snr_power, size_t scratch_bytes)
+{
+  char why[240];
+  if (awm_batch_rates_validate (items, n_items, n_values, sample_rates, n_emit, mark_sample_rate, why, sizeof (why)))
+    return fail (ctx, "awm_embed_batch_rates: %s", why);
+  if (!ctx->roles_fpb)
+    return fail (ctx, "awm_embed_batch_rates: awm_set_embed_roles has not been called");
+  if ((n_items && (!coded_bits || !n_emit)) || (n_values && (!in_v || !out_v)) || limiter_ms < 0)
+    return fail (ctx, "awm_embed_batch_rates: bad arguments");
+  if (snr_power)
+    std::fill (snr_power, snr_power + 2 * n_items, 0.0);
+  if (n_values == 0)
+    return 0;
+  CK (cudaSetDevice (ctx->device));
+  const bool s16 = is_s16 != 0;
+  const float *d_in;
+  float *d_out;
+  if (batch_images (ctx, in_v, out_v, s16, n_values, &d_in, &d_out))
+    return 1;
+  auto block_of = [&] (int rate) { return int ((long long) rate * limiter_ms / 1000); };      // add_watermark_buffer's limiter block
+
+  /* filter tables of every resampled rate, all fetched before any is used: coef_table empties its cache when it is full */
+  struct Filters { const float *coef_in = nullptr, *coef_out = nullptr; int h_in = 0, h_out = 0; };
+  std::map<int, Filters> filters;
+  for (size_t i = 0; i < n_items; i++)
+    if (items[i].n_frames && sample_rates[i] != mark_sample_rate)
+      filters[sample_rates[i]];
+  if (coef_cache_room (ctx, 2 * filters.size()))
+    return 1;
+  for (auto& f : filters)
+    if (coef_table (ctx, double (mark_sample_rate) / f.first, 16, &f.second.coef_in, &f.second.h_in) ||
+        coef_table (ctx, double (f.first) / mark_sample_rate, 16, &f.second.coef_out, &f.second.h_out))
+      return 1;
+
+  /* work lists.  Items at the watermark rate: one k_embed_batch pass as in awm_embed_batch.  The others: consecutive waves whose
+   * scratch (input and watermark signal at the watermark rate, 2 x n44 x C floats per item) stays within scratch_bytes; an item
+   * larger than that runs alone.  A wave's scratch holds the inputs of all its items, then their watermark signals. */
+  struct Wave { size_t b0 = 0, r0 = 0, r1 = 0, values = 0; long long n_tiles = 0, n_rs = 0, n_mix = 0, n_lim = 0; };
+  std::vector<BatchItem> blist;
+  std::vector<RateItem> rlist;
+  std::vector<size_t> soff;                 // offset of rlist[k] in its wave's input half of the scratch
+  std::vector<Wave> waves;
+  const int block44 = block_of (mark_sample_rate);
+  long long n_tiles44 = 0, n_lim44 = 0, n_peaks = 0, unused = 0;
+  uint64_t covered = 0;
+  for (size_t i = 0; i < n_items; i++)
+    {
+      covered += items[i].n_frames * uint64_t (items[i].channels);
+      if (items[i].n_frames && sample_rates[i] == mark_sample_rate)
+        blist.push_back (batch_entry ((long long) items[i].value_offset, (long long) items[i].n_frames, items[i].channels, int (i), block44,
+                                      n_tiles44, n_lim44, n_peaks));
+    }
+  const size_t n_list44 = blist.size();
+  const size_t cap = scratch_bytes ? scratch_bytes : kBatchDefaultScratch;
+  size_t max_values = 0;
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const awm_batch_item& bi = items[i];
+      const int rate = sample_rates[i];
+      if (!bi.n_frames || rate == mark_sample_rate)
+        continue;
+      const Filters& f = filters[rate];
+      RateItem R = {};
+      R.in = d_in + bi.value_offset;
+      R.out = d_out + bi.value_offset;
+      R.n_frames = (long long) bi.n_frames;
+      R.n_emit = (long long) n_emit[i];
+      R.C = bi.channels;
+      R.item = int (i);
+      R.step_in = 1.0 / (double (mark_sample_rate) / rate);      // as awm_embed_resampled: 1 / r_in, 1 / r_out
+      R.step_out = 1.0 / (double (rate) / mark_sample_rate);
+      R.h_in = f.h_in;
+      R.h_out = f.h_out;
+      R.coef_in = f.coef_in;
+      R.coef_out = f.coef_out;
+      R.n44 = resampled_n44 (n_emit[i], R.step_out, R.h_out);
+      R.limiter_block = block_of (rate);
+      R.n_blocks = R.limiter_block > 0 ? (R.n_emit + R.limiter_block - 1) / R.limiter_block + 1 : 0;   // as awm_embed_resampled's
+      R.peak0 = n_peaks;
+      n_peaks += R.n_blocks;
+      const size_t values = size_t (R.n44) * size_t (R.C);
+      if (waves.empty() || (waves.back().r1 > waves.back().r0 && 2 * (waves.back().values + values) * sizeof (float) > cap))
+        {
+          Wave w;
+          w.b0 = blist.size();
+          w.r0 = w.r1 = rlist.size();
+          waves.push_back (w);
+        }
+      Wave& w = waves.back();
+      R.rs0 = w.n_rs;
+      R.mix0 = w.n_mix;
+      R.lim0 = w.n_lim;
+      w.n_rs += (R.n44 + kRateCta - 1) / kRateCta;
+      w.n_mix += (R.n_emit + kRateCta - 1) / kRateCta;
+      if (R.limiter_block > 0)
+        w.n_lim += (R.n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter);
+      /* WatermarkGen::run on the scratch copy: awm_embed_resampled's k_embed with n_frames = n44, no limiter, no --snr */
+      blist.push_back (batch_entry ((long long) w.values, R.n44, R.C, int (i), 0, w.n_tiles, unused, unused));
+      soff.push_back (w.values);
+      w.values += values;
+      rlist.push_back (R);
+      w.r1 = rlist.size();
+      max_values = std::max (max_values, w.values);
+    }
+  bool too_large = n_tiles44 >= INT_MAX || n_lim44 >= INT_MAX || blist.size() >= size_t (INT_MAX);
+  for (const Wave& w : waves)
+    too_large = too_large || std::max ({ w.n_tiles, w.n_rs, w.n_mix, w.n_lim }) >= INT_MAX;
+  if (too_large)
+    return fail (ctx, "awm_embed_batch_rates: batch too large for one launch per step");
+  if (covered < n_values)               /* values between items pass through unchanged */
+    CK (cudaMemcpyAsync (d_out, d_in, n_values * sizeof (float), cudaMemcpyDeviceToDevice, ctx->stream));
+  if (!blist.empty())
+    {
+      if (!rlist.empty())
+        {
+          CK (ctx->rate_scratch.reserve (2 * max_values * sizeof (float)));
+          for (const Wave& w : waves)
+            for (size_t k = w.r0; k < w.r1; k++)
+              {
+                rlist[k].x44 = ctx->rate_scratch.as<float>() + soff[k];
+                rlist[k].wm44 = rlist[k].x44 + w.values;
+              }
+          CK (ctx->rate_items.reserve (rlist.size() * sizeof (RateItem)));
+          CK (cudaMemcpyAsync (ctx->rate_items.p, rlist.data(), rlist.size() * sizeof (RateItem), cudaMemcpyHostToDevice, ctx->stream));
+        }
+      const size_t coded_bytes = n_items * 2 * size_t (ctx->roles_n_coded);
+      CK (ctx->batch_items.reserve (blist.size() * sizeof (BatchItem)));
+      CK (ctx->batch_coded.reserve (coded_bytes));
+      CK (cudaMemcpyAsync (ctx->batch_items.p, blist.data(), blist.size() * sizeof (BatchItem), cudaMemcpyHostToDevice, ctx->stream));
+      CK (cudaMemcpyAsync (ctx->batch_coded.p, coded_bits, coded_bytes, cudaMemcpyHostToDevice, ctx->stream));
+      if (n_peaks)
+        {
+          CK (ctx->peaks.reserve (n_peaks * sizeof (unsigned)));
+          CK (cudaMemsetAsync (ctx->peaks.p, 0, n_peaks * sizeof (unsigned), ctx->stream));
+        }
+      if (snr_power)
+        {
+          CK (ctx->snr.reserve (2 * n_items * sizeof (double)));
+          CK (cudaMemsetAsync (ctx->snr.p, 0, 2 * n_items * sizeof (double), ctx->stream));
+        }
+      double *d_snr = snr_power ? ctx->snr.as<double>() : nullptr;
+      const BatchItem *d_b = ctx->batch_items.as<BatchItem>();
+      if (n_list44 && launch_embed_batch (ctx, d_in, d_out, d_b, int (n_list44), n_tiles44, n_lim44, frames_pad_start, water_delta, block44,
+                                          limiter_ceiling, d_snr, 0))
+        return 1;
+      for (const Wave& w : waves)
+        {
+          const RateItem *d_r = ctx->rate_items.as<RateItem>() + w.r0;
+          const int n_r = int (w.r1 - w.r0);
+          float *x44 = ctx->rate_scratch.as<float>();
+          PROF (ctx);
+          k_resample_batch<<<unsigned (w.n_rs), kRateCta, 0, ctx->stream>>> (d_r, n_r);
+          LAUNCH_CHECK ("k_resample_batch");
+          if (launch_embed_batch (ctx, x44, x44 + w.values, d_b + w.b0, n_r, w.n_tiles, 0, frames_pad_start, water_delta, 0, limiter_ceiling, nullptr, 1))
+            return 1;
+          PROF (ctx);
+          k_resample_mix_batch<<<unsigned (w.n_mix), kRateCta, 0, ctx->stream>>> (d_r, n_r, limiter_ceiling, ctx->peaks.as<unsigned>(), d_snr);
+          LAUNCH_CHECK ("k_resample_mix_batch");
+          if (w.n_lim)
+            {
+              PROF (ctx);
+              k_limiter_rates<<<unsigned (w.n_lim), 256, 0, ctx->stream>>> (d_r, n_r, limiter_ceiling, ctx->peaks.as<unsigned>());
+              LAUNCH_CHECK ("k_limiter_rates");
+            }
+        }
+    }
+  return batch_finish (ctx, out_v, s16, n_values, d_out, snr_power, blist.empty() ? 0 : n_items);
 }
 
 /* ---------------------------------------------------------------- speed scan */

@@ -32,60 +32,90 @@ struct ResampleJob
 // out[n] = sum_j x[c - 2h + 2 + j] * ((1-a) coef[p][j] + a coef[p+1][j]),  t = (h-1) + n step, c = floor t,
 // (p, a) = integer / fractional part of 256 (t - c); x is zero outside [0, n_in).  Float products and sums are kept
 // separate and in tap order, t is evaluated in closed form in double: a sequential implementation that does the same
-// gets the same bits.
+// gets the same bits.  resample_pos / resample_dot2 / resample_dot are that arithmetic for one output frame; k_resample and
+// the batched kernels (awm_batch_rates.cuh) share them, so every caller produces the same bits.
+struct ResamplePos
+{
+  long long i0;             // input frame of the first tap
+  const float *c0;          // phase row p of the table (row p + 1 follows)
+  float a, b;               // interpolation weights of rows p + 1 and p
+};
+
+// false: output n is 0 (its taps would run past the post-roll, where a streaming resampler stops)
+__device__ __forceinline__ bool
+resample_pos (const ResampleJob& J, long long n, ResamplePos& P)
+{
+  const int h = J.h;
+  const double t = __dadd_rn (double (h - 1), __dmul_rn (double (n), J.step));
+  const double fl = floor (t);
+  const long long c = (long long) fl;
+  if (c > J.n_stop + h - 2)
+    return false;
+  const double frac = __dmul_rn (__dsub_rn (t, fl), double (kResamplePhases));
+  const int p = int (frac);
+  P.a = float (__dsub_rn (frac, double (p)));
+  P.b = __fsub_rn (1.0f, P.a);
+  P.c0 = J.coef + p;
+  P.i0 = c - 2LL * h + 2;
+  return true;
+}
+
+// both channels of a stereo output; J.in must be 8-byte aligned
+__device__ __forceinline__ float2
+resample_dot2 (const ResampleJob& J, const ResamplePos& P)
+{
+  constexpr int RS = kResamplePhases + 1;        // row stride of the tap-major table
+  const float *c0 = P.c0, *c1 = c0 + 1;
+  const float2 *x2 = reinterpret_cast<const float2 *> (J.in);
+  float s0 = 0.0f, s1 = 0.0f;
+  for (int j = 0; j < 2 * J.h; j++)
+    {
+      const long long i = P.i0 + j;
+      const float w = __fadd_rn (__fmul_rn (P.b, __ldg (c0 + j * RS)), __fmul_rn (P.a, __ldg (c1 + j * RS)));
+      const float2 x = (i >= 0 && i < J.n_in) ? __ldg (x2 + i) : make_float2 (0.0f, 0.0f);
+      s0 = __fadd_rn (s0, __fmul_rn (x.x, w));
+      s1 = __fadd_rn (s1, __fmul_rn (x.y, w));
+    }
+  return make_float2 (s0, s1);
+}
+
+// channel ch of an output of CH interleaved channels
+__device__ __forceinline__ float
+resample_dot (const ResampleJob& J, const ResamplePos& P, int CH, int ch)
+{
+  constexpr int RS = kResamplePhases + 1;
+  const float *c0 = P.c0, *c1 = c0 + 1;
+  float s = 0.0f;
+  for (int j = 0; j < 2 * J.h; j++)
+    {
+      const long long i = P.i0 + j;
+      const float w = __fadd_rn (__fmul_rn (P.b, __ldg (c0 + j * RS)), __fmul_rn (P.a, __ldg (c1 + j * RS)));
+      const float x = (i >= 0 && i < J.n_in) ? __ldg (J.in + i * CH + ch) : 0.0f;
+      s = __fadd_rn (s, __fmul_rn (x, w));
+    }
+  return s;
+}
+
 template<int C> __global__ void __launch_bounds__ (256)
 k_resample (const ResampleJob *__restrict__ jobs, int c_dyn)
 {
   const ResampleJob J = jobs[blockIdx.y];
   const int CH = C > 0 ? C : c_dyn;
-  const int h = J.h, taps = 2 * h;
   for (long long n = (long long) blockIdx.x * blockDim.x + threadIdx.x; n < J.n_out; n += (long long) gridDim.x * blockDim.x)
     {
-      const double t = __dadd_rn (double (h - 1), __dmul_rn (double (n), J.step));
-      const double fl = floor (t);
-      const long long c = (long long) fl;
       float *o = J.out + n * CH;
-      if (c > J.n_stop + h - 2)                  // taps would run past the post-roll: a streaming resampler stops here
+      ResamplePos P;
+      if (!resample_pos (J, n, P))
         {
           for (int ch = 0; ch < CH; ch++)
             o[ch] = 0.0f;
           continue;
         }
-      const double frac = __dmul_rn (__dsub_rn (t, fl), double (kResamplePhases));
-      const int p = int (frac);
-      const float a = float (__dsub_rn (frac, double (p))), b = __fsub_rn (1.0f, a);
-      const float *c0 = J.coef + p, *c1 = c0 + 1;
-      constexpr int RS = kResamplePhases + 1;        // row stride of the tap-major table
-      const long long i0 = c - 2LL * h + 2;
       if (C == 2)
-        {
-          float s0 = 0.0f, s1 = 0.0f;
-          const float2 *x2 = reinterpret_cast<const float2 *> (J.in);
-          for (int j = 0; j < taps; j++)
-            {
-              const long long i = i0 + j;
-              const float w = __fadd_rn (__fmul_rn (b, __ldg (c0 + j * RS)), __fmul_rn (a, __ldg (c1 + j * RS)));
-              const float2 x = (i >= 0 && i < J.n_in) ? __ldg (x2 + i) : make_float2 (0.0f, 0.0f);
-              s0 = __fadd_rn (s0, __fmul_rn (x.x, w));
-              s1 = __fadd_rn (s1, __fmul_rn (x.y, w));
-            }
-          reinterpret_cast<float2 *> (J.out)[n] = make_float2 (s0, s1);
-        }
+        reinterpret_cast<float2 *> (J.out)[n] = resample_dot2 (J, P);
       else
-        {
-          for (int ch = 0; ch < CH; ch++)
-            {
-              float s = 0.0f;
-              for (int j = 0; j < taps; j++)
-                {
-                  const long long i = i0 + j;
-                  const float w = __fadd_rn (__fmul_rn (b, __ldg (c0 + j * RS)), __fmul_rn (a, __ldg (c1 + j * RS)));
-                  const float x = (i >= 0 && i < J.n_in) ? __ldg (J.in + i * CH + ch) : 0.0f;
-                  s = __fadd_rn (s, __fmul_rn (x, w));
-                }
-              o[ch] = s;
-            }
-        }
+        for (int ch = 0; ch < CH; ch++)
+          o[ch] = resample_dot (J, P, CH, ch);
     }
 }
 

@@ -205,6 +205,66 @@ add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t
   return 0;
 }
 
+int
+add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                           const vector<string>& bits, const int *sample_rates, size_t scratch_bytes, vector<AddStats> *stats)
+{
+  char why[256];
+  if (awm_batch_rates_validate (items, n_items, n_values, sample_rates, nullptr, Params::mark_sample_rate, why, sizeof (why)))
+    {
+      error ("audiowmark: %s\n", why);
+      return 2;
+    }
+  vector<uint8_t> coded;
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const vector<int> bitvec = parse_payload (bits[i]);
+      if (bitvec.empty())
+        return 2;
+      const vector<uint8_t> c = gen_coded_bits (key, bitvec);
+      coded.insert (coded.end(), c.begin(), c.end());
+    }
+  /* per item what add_watermark_buffer computes for it: frames through the mixer (other rates) and WatermarkGen::run calls */
+  vector<uint64_t> n_emit (n_items);
+  vector<size_t> runs (n_items);
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const int rate = sample_rates[i];
+      const size_t block = size_t (rate) * size_t (Params::limiter_block_size_ms) / 1000;
+      if (rate == Params::mark_sample_rate)
+        {
+          runs[i] = gen_runs (items[i].n_frames, !Params::test_no_limiter, block);
+          continue;
+        }
+      size_t emit = 0;
+      resampled_add_plan (items[i].n_frames, rate, !Params::test_no_limiter, block, emit, runs[i]);
+      n_emit[i] = std::max<uint64_t> (emit, items[i].n_frames);
+    }
+  awm_ctx *ctx = Engine::ctx();
+  if (!ctx || !Engine::set_embed_roles (key))
+    return 1;
+  vector<double> snr_power (2 * n_items);
+  if (awm_embed_batch_rates (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), Params::mark_sample_rate,
+                             Params::frames_pad_start, Params::water_delta, Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms),
+                             Params::limiter_ceiling, (Params::snr || stats) ? snr_power.data() : nullptr, scratch_bytes))
+    {
+      error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
+      return 1;
+    }
+  if (stats)
+    {
+      stats->resize (n_items);
+      const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
+      for (size_t i = 0; i < n_items; i++)
+        {
+          const int blocks = int ((f0 + runs[i]) / fpb - f0 / fpb);
+          (*stats)[i].data_blocks = std::max (blocks - 1, 0);
+          (*stats)[i].snr_db = snr_power[2 * i] > 0 ? 10 * log10 (snr_power[2 * i + 1] / snr_power[2 * i]) : INFINITY;
+        }
+    }
+  return 0;
+}
+
 /* Part of the stream a window has to embed so that [own_start, own_end) comes out exactly as in a run over the whole stream:
  * one 1024-frame before the first limiter block that influences the owned range (synthesis-window tail of the frame before) and
  * everything up to the end of the limiter block after the last owned one (the gain ramp looks one block ahead), rounded to whole

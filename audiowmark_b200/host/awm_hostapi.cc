@@ -296,6 +296,41 @@ awmh_add_batch_s16 (const unsigned char *key16, const int16_t *in, int16_t *out,
   return add_batch_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db);
 }
 
+/* add_watermark_batch_rates on a packed buffer: items[i] is at sample_rates[i]; otherwise as awmh_add_batch */
+static int
+add_batch_rates_any (const unsigned char *key16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                     const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db)
+{
+  std::vector<std::string> bits (n_items);
+  for (size_t i = 0; i < n_items; i++)
+    bits[i] = payload_hex[i] ? payload_hex[i] : "";
+  std::vector<AddStats> stats;
+  const int rc = add_watermark_batch_rates (make_key (key16, ""), in, out, s16, n_values, items, n_items, bits, sample_rates, scratch_bytes,
+                                            (data_blocks || snr_db) ? &stats : nullptr);
+  for (size_t i = 0; i < stats.size(); i++)
+    {
+      if (data_blocks)
+        data_blocks[i] = stats[i].data_blocks;
+      if (snr_db)
+        snr_db[i] = stats[i].snr_db;
+    }
+  return rc;
+}
+
+int
+awmh_add_batch_rates (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                      const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db)
+{
+  return add_batch_rates_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
+}
+
+int
+awmh_add_batch_rates_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                          const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db)
+{
+  return add_batch_rates_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
+}
+
 /* add / get between 16 bit PCM host buffers (the contents of a 16 bit WAV file): conversions run on the device */
 int
 awmh_add_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_frames, int n_channels, int sample_rate,

@@ -17,7 +17,7 @@ CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
            "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_add_windowed",
-           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16"]
+           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16", "awmh_add_batch_rates", "awmh_add_batch_rates_s16"]
 
 _lib = None
 
@@ -182,15 +182,9 @@ def add(pcm_in, payload_hex: str, key=None, pcm_out=None, n_frames=None, channel
     return (pcm_out, blocks.value, snr.value) if want_stats else pcm_out
 
 
-def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False):
-    """`add` for many items with one key and one payload each, in one pass over the GPU; item i comes out bit identical to
-    add / add_s16 of that item alone with payloads[i].
-      pcms: a list of numpy arrays [n, channels] (all float32 or all int16; channels may differ), or one packed device tensor
-            (float32 or int16, contiguous) with items = [(value_offset, n_frames, channels), ...] in values of that tensor;
-            out: a device tensor like pcms for the result (default: a new one).
-    Returns the list of outputs (numpy arrays, or views of the output tensor), with want_stats also the lists of data blocks
-    and SNR dB per item.  Only 44.1 kHz input is accepted.  Raises ValueError for a malformed item list or payload."""
-    payloads = list(payloads)
+def _pack_batch(name, pcms, payloads, items, out):
+    """the packed buffers of a batch call -> (s16, item array, n_values, in pointer, out pointer, split (offset, frames, channels) ->
+    output view, buffers to keep alive); see add_batch for the two input forms"""
     if items is None:
         arrays = [np.asarray(p) for p in pcms]
         s16 = bool(arrays) and all(a.dtype == np.int16 for a in arrays)
@@ -208,18 +202,32 @@ def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None,
     else:
         import torch
         if not (pcms.is_cuda and pcms.is_contiguous() and pcms.dtype in (torch.float32, torch.int16)):
-            raise ValueError("add_batch: pcms must be a contiguous float32 or int16 CUDA tensor")
+            raise ValueError("%s: pcms must be a contiguous float32 or int16 CUDA tensor" % name)
         s16 = pcms.dtype == torch.int16
         res = torch.empty_like(pcms) if out is None else out
         if res.dtype != pcms.dtype or res.numel() != pcms.numel() or not res.is_contiguous():
-            raise ValueError("add_batch: out must be a contiguous tensor like pcms")
+            raise ValueError("%s: out must be a contiguous tensor like pcms" % name)
         flat = res.view(-1)
         torch.cuda.current_stream(pcms.device).synchronize()      # the context works on its own stream
         n_values, p_in, p_out = pcms.numel(), ctypes.c_void_p(pcms.data_ptr()), ctypes.c_void_p(res.data_ptr())
         split = lambda o, n, c: flat[o:o + n * c].view(n, c)
+        packed = pcms
     if len(payloads) != len(items):
-        raise ValueError("add_batch: %d items but %d payloads" % (len(items), len(payloads)))
+        raise ValueError("%s: %d items but %d payloads" % (name, len(items), len(payloads)))
     it = np.array([tuple(int(v) for v in t) for t in items], capi.BATCH_ITEM)
+    return s16, it, n_values, p_in, p_out, split, (packed, res)
+
+
+def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False):
+    """`add` for many items with one key and one payload each, in one pass over the GPU; item i comes out bit identical to
+    add / add_s16 of that item alone with payloads[i].
+      pcms: a list of numpy arrays [n, channels] (all float32 or all int16; channels may differ), or one packed device tensor
+            (float32 or int16, contiguous) with items = [(value_offset, n_frames, channels), ...] in values of that tensor;
+            out: a device tensor like pcms for the result (default: a new one).
+    Returns the list of outputs (numpy arrays, or views of the output tensor), with want_stats also the lists of data blocks
+    and SNR dB per item.  Only 44.1 kHz input is accepted.  Raises ValueError for a malformed item list or payload."""
+    payloads = list(payloads)
+    s16, it, n_values, p_in, p_out, split, _keep = _pack_batch("add_batch", pcms, payloads, items, out)
     pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
     blocks = np.zeros(max(len(it), 1), np.int32)
     snr = np.zeros(max(len(it), 1), np.float64)
@@ -230,6 +238,35 @@ def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None,
         raise ValueError("add_batch: malformed item list or payload; see stderr")
     if rc:
         raise RuntimeError("awmh_add_batch failed (rc=%d); see stderr" % rc)
+    synchronize()
+    outs = [split(int(t["value_offset"]), int(t["n_frames"]), int(t["channels"])) for t in it]
+    return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs
+
+
+def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None, want_stats=False, scratch_bytes=0):
+    """add_batch for items that each have their own sample rate: item i comes out bit identical to add(item, payloads[i],
+    sample_rate=sample_rates[i]) of that item alone (16 bit items: to that `add` between int16_to_float and 16 bit quantisation, what
+    `audiowmark add` computes on a 16 bit file).  pcms / items / out / want_stats as in add_batch.  scratch_bytes: device scratch
+    per wave of resampled items (0: the library's default of 4 GiB; a smaller value runs more, smaller waves with the same result).
+    Raises ValueError for a malformed item list, rate list or payload."""
+    payloads = list(payloads)
+    rates = np.array([int(r) for r in sample_rates], np.int64)
+    s16, it, n_values, p_in, p_out, split, _keep = _pack_batch("add_batch_rates", pcms, payloads, items, out)
+    if len(rates) != len(it):
+        raise ValueError("add_batch_rates: %d items but %d sample rates" % (len(it), len(rates)))
+    if np.any(rates <= 0) or np.any(rates > np.iinfo(np.int32).max):
+        raise ValueError("add_batch_rates: sample rates must be positive 32 bit integers")
+    rates = np.ascontiguousarray(rates, np.int32)
+    pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
+    blocks = np.zeros(max(len(it), 1), np.int32)
+    snr = np.zeros(max(len(it), 1), np.float64)
+    fn = load().awmh_add_batch_rates_s16 if s16 else load().awmh_add_batch_rates
+    rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, _ptr(rates),
+            ctypes.c_size_t(scratch_bytes), _ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
+    if rc == 2:
+        raise ValueError("add_batch_rates: malformed item list, sample rate or payload; see stderr")
+    if rc:
+        raise RuntimeError("awmh_add_batch_rates failed (rc=%d); see stderr" % rc)
     synchronize()
     outs = [split(int(t["value_offset"]), int(t["n_frames"]), int(t["channels"])) for t in it]
     return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs

@@ -182,12 +182,27 @@ int awm_batch_validate (const awm_batch_item *items, size_t n_items, size_t n_va
 /* awm_embed (first_frame_number 0) for every item of a packed buffer in one pass: item i comes out bit identical to awm_embed /
  * awm_embed_s16 on that item alone with the FrameMod table of payload i.  in / out: n_values floats (is_s16 = 0) or int16
  * (is_s16 = 1), host or device; host buffers cross PCIe as one copy each way.  Items must not overlap.  Values of out that belong
- * to no item are copied from in when out is host memory and left alone when it is device memory.
+ * to no item are copied from in.
  * coded_bits: uint8 [n_items][2 (A, B)][n_coded_bits] (randomize_bit_order (code_encode (A | B, payload))).
  * snr_power (optional): [n_items][2] as awm_embed's.  Roles come from awm_set_embed_roles; zero items and zero-length items are legal. */
 int awm_embed_batch (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
                      const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
                      double *snr_power);
+/* 0 if awm_batch_validate passes, mark_sample_rate > 0, every sample_rates[i] > 0, every rate other than mark_sample_rate has both
+ * resampling ratios (mark / rate, rate / mark) inside the resampler's range (1/64, 64), at most 256 such rates are distinct and, where
+ * n_emit is not NULL, n_emit[i] >= n_frames of every resampled item; else nonzero with the reason in err.  Needs no device. */
+int awm_batch_rates_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const int *sample_rates, const uint64_t *n_emit,
+                              int mark_sample_rate, char *err, size_t err_cap);
+/* awm_embed_batch for items that each have their own sample rate.  Item i comes out bit identical to what `add` of that item alone
+ * computes: awm_embed for sample_rates[i] == mark_sample_rate, awm_embed_resampled (n_emit[i], limiter block
+ * sample_rates[i] * limiter_ms / 1000) for any other rate; 16 bit items as the float path between k_s16_to_f32 and k_f32_to_s16.
+ * n_emit: [n_items], the frames awm_embed_resampled takes (resampled_add_plan on the host); ignored at mark_sample_rate.
+ * limiter_ms = 0 disables the limiter.  snr_power (optional): [n_items][2].  Items at other rates run in consecutive waves whose
+ * scratch (2 x n44 x channels floats per item, n44 = its length at mark_sample_rate) stays within scratch_bytes (0: 4 GiB); an item
+ * larger than that runs alone.  The bound PCM (awm_pcm_bind) stays valid.  Everything else as awm_embed_batch. */
+int awm_embed_batch_rates (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                           const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate, int frames_pad_start,
+                           double water_delta, int limiter_ms, float limiter_ceiling, double *snr_power, size_t scratch_bytes);
 
 /* ---- sync search on the bound PCM --------------------------------------------------------
  * awm_sync_approx = SyncFinder::search_approx (src/syncfinder.cc:171-256): for the four
