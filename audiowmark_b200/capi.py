@@ -29,7 +29,7 @@ EXPORTS = [
     "awm_create", "awm_destroy", "awm_last_error", "awm_launch_count", "awm_stream", "awm_synchronize",
     "awm_profile_enable", "awm_profile_report", "awm_host_alloc", "awm_host_free",
     "awm_fft_r2c", "awm_fft_c2r", "awm_set_embed_tables", "awm_set_sync_tables", "awm_set_mix_tables",
-    "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_decode_blocks", "awm_viterbi",
+    "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_approx_enqueue", "awm_sync_use_slot", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_sync_refine_rescored", "awm_decode_blocks", "awm_viterbi",
     "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_is_device_pointer", "awm_speed_scan", "awm_embed_resampled", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_prefetch_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
     "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch", "awm_batch_rates_validate", "awm_embed_batch_rates",
 ]
@@ -250,6 +250,16 @@ class Context:
         self._ck(self.lib.awm_sync_refine_offsets(self.h, ctypes.c_int(key_slot), ctypes.c_int(mode), ctypes.c_uint64(wav_first), ctypes.c_uint64(wav_last),
                                                   ctypes.c_double(water_delta), _ptr(s), ctypes.c_size_t(len(s)), ctypes.c_int(1 if exact else 0), _ptr(q), _ptr(valid)))
         return q, valid.astype(bool)
+
+    def sync_refine_rescored(self, scores: np.ndarray, key_slot=0, mode=MODE_BLOCK, wav_first=0, wav_last=None, water_delta=0.01):
+        """[n][65] bool: the fine offsets awm_sync_refine scores again exactly, as the device ranking picks them"""
+        if wav_last is None:
+            wav_last = 0xFFFFFFFFFFFFFFF
+        s = np.ascontiguousarray(scores, SEARCH_SCORE)
+        out = np.zeros((len(s), 65), np.uint8)
+        self._ck(self.lib.awm_sync_refine_rescored(self.h, ctypes.c_int(key_slot), ctypes.c_int(mode), ctypes.c_uint64(wav_first), ctypes.c_uint64(wav_last),
+                                                   ctypes.c_double(water_delta), _ptr(s), ctypes.c_size_t(len(s)), _ptr(out)))
+        return out.astype(bool)
 
     # ---- decode
     def decode_blocks(self, indices, n_coded: int, key_slot=0):

@@ -166,9 +166,21 @@ struct awm_ctx
   int stage_ch = 0;
   bool stage_s16 = false;
 
-  DevBuf dbT, have, q, scores, a_ud, a_cnt, peaks_out, peaks_cnt, a_mags;       // approx
-  size_t n_scores_dev = 0;
+  /* approx: the per-call state of awm_sync_approx lives in a slot, so that the search of the next chunk can run
+   * (awm_sync_approx_enqueue, on s_approx) while peaks / refine / decode of the current one read theirs */
+  struct ApproxSlot
+  {
+    DevBuf have, q, scores, a_ud, a_cnt;
+    size_t n_scores = 0;
+    const float *pcm = nullptr; size_t pcm_frames = 0; int pcm_ch = 0;    // the PCM view the search ran on
+    cudaEvent_t done = nullptr;                                           // recorded after k_local_mean
+  };
+  ApproxSlot aslot[2];
+  int cur_aslot = 0;
+  cudaStream_t s_approx = nullptr;
+  DevBuf dbT, peaks_out, peaks_cnt, a_mags;   // a_mags is shared: every slot's gather runs before the next search overwrites it
   DevBuf cand_start, cand_noff, r_ud, r_cnt, rvalid, r_ent_ud, r_ent_flag, tw1024;   // refine
+  DevBuf cand_score, rank_keep, rank_first, ex_start, ex_cand, ex_off, ex_n;         // offsets picked for exact re-scoring (k_refine_rank)
   DevBuf blk_start, D, raw;          // decode
   DevBuf vit_raw, vit_off, vit_types, vit_delta, vit_dec, vit_bits, vit_err;
   DevBuf emb_in, emb_out, emb_in16, emb_out16, peaks, snr;
@@ -364,8 +376,11 @@ awm_destroy (awm_ctx *ctx)
     return;
   cudaSetDevice (ctx->device);
   cudaStreamSynchronize (ctx->stream);
-  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->rate_items, &ctx->rate_scratch, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->have, &ctx->q, &ctx->scores, &ctx->a_ud, &ctx->a_cnt, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
-                     &ctx->cand_start, &ctx->cand_noff, &ctx->r_ud, &ctx->r_cnt, &ctx->rvalid, &ctx->r_ent_ud, &ctx->r_ent_flag, &ctx->tw1024, &ctx->vit_off, &ctx->blk_start, &ctx->D, &ctx->raw,
+  if (ctx->s_approx)
+    cudaStreamSynchronize (ctx->s_approx);
+  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->rate_items, &ctx->rate_scratch, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
+                     &ctx->cand_start, &ctx->cand_noff, &ctx->r_ud, &ctx->r_cnt, &ctx->rvalid, &ctx->r_ent_ud, &ctx->r_ent_flag, &ctx->tw1024,
+                     &ctx->cand_score, &ctx->rank_keep, &ctx->rank_first, &ctx->ex_start, &ctx->ex_cand, &ctx->ex_off, &ctx->ex_n, &ctx->vit_off, &ctx->blk_start, &ctx->D, &ctx->raw,
                      &ctx->vit_raw, &ctx->vit_types, &ctx->vit_delta, &ctx->vit_dec, &ctx->vit_bits, &ctx->vit_err,
                      &ctx->emb_in, &ctx->emb_out, &ctx->emb_in16, &ctx->emb_out16, &ctx->peaks, &ctx->snr, &ctx->rs_in, &ctx->rs_out, &ctx->rs_jobs, &ctx->pcm_rs,
                      &ctx->win512, &ctx->sp_clip, &ctx->sp_sub, &ctx->sp_mags, &ctx->sp_mag_jobs, &ctx->sp_cmp_jobs, &ctx->sp_best };
@@ -400,8 +415,18 @@ awm_destroy (awm_ctx *ctx)
       k.mix.release();
       k.order.release();
     }
+  for (auto& s : ctx->aslot)
+    {
+      DevBuf *sb[] = { &s.have, &s.q, &s.scores, &s.a_ud, &s.a_cnt };
+      for (DevBuf *b : sb)
+        b->release();
+      if (s.done)
+        cudaEventDestroy (s.done);
+    }
   for (cudaEvent_t e : ctx->stage_done)
     cudaEventDestroy (e);
+  if (ctx->s_approx)
+    cudaStreamDestroy (ctx->s_approx);
   if (ctx->s_in)
     cudaStreamDestroy (ctx->s_in);
   if (ctx->s_out)
@@ -1447,9 +1472,12 @@ awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t
 
 /* ---------------------------------------------------------------- sync search */
 
+namespace {
+
+/* the search of awm_sync_approx on the bound PCM into approx slot `s`, on ctx->stream */
 int
-awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last,
-                 double water_delta, awm_search_score *scores_out, size_t max_scores, size_t *n_scores)
+approx_launch (awm_ctx *ctx, awm_ctx::ApproxSlot& s, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last,
+               double water_delta, awm_search_score *scores_out, size_t max_scores, size_t *n_scores)
 {
   if (key_slot < 0 || key_slot >= AWM_MAX_KEYS || mode < 0 || mode > 1 || !n_scores)
     return fail (ctx, "awm_sync_approx: bad arguments");
@@ -1465,17 +1493,25 @@ awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
   const long long n_out = fc > 0 ? fc - 1 : 0;                           // sync_fft_parallel: frame_count - 1 frames per shift
   const long long n_starts = fc - total - 1 > 0 ? fc - total - 1 : 0;    // (start + total) * n_bands < fft_db.size()
   *n_scores = size_t (n_starts) * 4;
-  ctx->n_scores_dev = 0;
+  s.n_scores = 0;
+  s.pcm = ctx->pcm;
+  s.pcm_frames = ctx->pcm_frames;
+  s.pcm_ch = ctx->pcm_ch;
+  if (!s.done)
+    CK (cudaEventCreateWithFlags (&s.done, cudaEventDisableTiming));
   if (n_starts == 0)
-    return 0;
+    {
+      CK (cudaEventRecord (s.done, ctx->stream));
+      return 0;
+    }
   if (scores_out && max_scores < size_t (n_starts) * 4)
     return fail (ctx, "awm_sync_approx: scores_out too small (%zu < %lld)", max_scores, n_starts * 4);
   const int ld = int ((n_out + 127) / 128 * 128);
-  CK (ctx->have.reserve (size_t (4) * ld));
-  CK (ctx->q.reserve (size_t (n_starts) * 4 * sizeof (double)));
-  CK (ctx->a_ud.reserve (size_t (n_starts) * 4 * t.n_bits * 2 * sizeof (float)));
-  CK (ctx->a_cnt.reserve (size_t (n_starts) * 4 * t.n_bits * sizeof (int)));
-  CK (ctx->scores.reserve (size_t (n_starts) * 4 * sizeof (awm_search_score)));
+  CK (s.have.reserve (size_t (4) * ld));
+  CK (s.q.reserve (size_t (n_starts) * 4 * sizeof (double)));
+  CK (s.a_ud.reserve (size_t (n_starts) * 4 * t.n_bits * 2 * sizeof (float)));
+  CK (s.a_cnt.reserve (size_t (n_starts) * 4 * t.n_bits * sizeof (int)));
+  CK (s.scores.reserve (size_t (n_starts) * 4 * sizeof (awm_search_score)));
   const double norm_div = water_delta < 0.080 ? water_delta : 0.080;     // normalize_sync_quality, src/syncfinder.cc:90
   /* default: entry sums on the tensor cores (k_stft_mags_tc, awm_approx_tc.cuh) + one streaming gather.  AWM_APPROX selects the
    * test references: simt = the same entry sums on the fp32 pipes (k_stft_mags, awm_approx_mags.cuh); ring = the kernel that walks
@@ -1497,7 +1533,7 @@ awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
           PROF (ctx);
           k_stft_mags_tc<<<grid, (kTcFftWarps + kTcEpiWarps) * 32, kTcSmemBytes, ctx->stream>>> (ctx->pcm, (long long) ctx->pcm_frames,
             ctx->pcm_ch, int (n_out), ld, t.masks.as<unsigned char>(), t.n_ent, t.n_chunks, ctx->a_mags.as<float2>(),
-            ctx->have.as<unsigned char>(), (long long) wav_first, (long long) wav_last, ctx->tw.as<float2>(), ctx->win.as<float>(), tma_ok);
+            s.have.as<unsigned char>(), (long long) wav_first, (long long) wav_last, ctx->tw.as<float2>(), ctx->win.as<float>(), tma_ok);
           LAUNCH_CHECK ("k_stft_mags_tc");
           prof_bytes (ctx, double (ctx->pcm_frames) * ctx->pcm_ch * sizeof (float) + double (4) * t.n_ent * n_out * sizeof (float2));   /* PCM in, entry sums out */
         }
@@ -1508,7 +1544,7 @@ awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
         const unsigned grid = 4u * unsigned ((n_out + kMagTile - 1) / kMagTile);
         PROF (ctx);
         k_stft_mags<<<grid, kMagWarps2 * 32, smem, ctx->stream>>> (ctx->pcm, (long long) ctx->pcm_frames, ctx->pcm_ch, int (n_out), ld,
-                                                                  t.ent.as<awm_sync_entry>(), t.n_ent, ctx->a_mags.as<float2>(), ctx->have.as<unsigned char>(),
+                                                                  t.ent.as<awm_sync_entry>(), t.n_ent, ctx->a_mags.as<float2>(), s.have.as<unsigned char>(),
                                                                   (long long) wav_first, (long long) wav_last, ctx->tw.as<float2>(), ctx->win.as<float>());
         LAUNCH_CHECK ("k_stft_mags");
         prof_bytes (ctx, double (ctx->pcm_frames) * ctx->pcm_ch * sizeof (float) + double (4) * t.n_ent * n_out * sizeof (float2));   /* PCM in, entry sums out */
@@ -1516,11 +1552,11 @@ awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
       dim3 grid (unsigned ((n_starts + 255) / 256), 4);
       PROF (ctx);
       if (mode == AWM_MODE_CLIP)
-        k_sync_gather<true><<<grid, 256, 0, ctx->stream>>> (ctx->a_mags.as<float2>(), ctx->have.as<unsigned char>(), ld, int (n_starts), t.ent.as<awm_sync_entry>(), t.n_ent,
-                                                            t.off.as<int>(), t.n_bits, ctx->a_ud.as<float>(), ctx->a_cnt.as<int>());
+        k_sync_gather<true><<<grid, 256, 0, ctx->stream>>> (ctx->a_mags.as<float2>(), s.have.as<unsigned char>(), ld, int (n_starts), t.ent.as<awm_sync_entry>(), t.n_ent,
+                                                            t.off.as<int>(), t.n_bits, s.a_ud.as<float>(), s.a_cnt.as<int>());
       else
-        k_sync_gather<false><<<grid, 256, 0, ctx->stream>>> (ctx->a_mags.as<float2>(), ctx->have.as<unsigned char>(), ld, int (n_starts), t.ent.as<awm_sync_entry>(), t.n_ent,
-                                                             t.off.as<int>(), t.n_bits, ctx->a_ud.as<float>(), ctx->a_cnt.as<int>());
+        k_sync_gather<false><<<grid, 256, 0, ctx->stream>>> (ctx->a_mags.as<float2>(), s.have.as<unsigned char>(), ld, int (n_starts), t.ent.as<awm_sync_entry>(), t.n_ent,
+                                                             t.off.as<int>(), t.n_bits, s.a_ud.as<float>(), s.a_cnt.as<int>());
       LAUNCH_CHECK ("k_sync_gather");
       /* every (start frame, entry) pair reads its float2 once; the per-bit sums are written once */
       prof_bytes (ctx, double (4) * n_starts * t.n_ent * sizeof (float2) + double (4) * n_starts * t.n_bits * 12.0);
@@ -1534,7 +1570,7 @@ awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
         const unsigned grid = 4u * unsigned ((n_out + kStftWarps - 1) / kStftWarps);
         PROF (ctx);
         k_stft_db<<<grid, kStftWarps * 32, smem, ctx->stream>>> (ctx->pcm, (long long) ctx->pcm_frames, ctx->pcm_ch, int (n_out), ld,
-                                                                ctx->dbT.as<float>(), ctx->have.as<unsigned char>(),
+                                                                ctx->dbT.as<float>(), s.have.as<unsigned char>(),
                                                                 (long long) wav_first, (long long) wav_last,
                                                                 ctx->tw.as<float2>(), ctx->win.as<float>());
         LAUNCH_CHECK ("k_stft_db");
@@ -1546,39 +1582,99 @@ awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
           {
             if (set_smem (ctx, k_sync_approx<true>, smem)) return 1;
             PROF (ctx);
-            k_sync_approx<true><<<grid, kApproxThreads, smem, ctx->stream>>> (ctx->dbT.as<float>(), ctx->have.as<unsigned char>(), ld, int (n_out), int (n_starts),
+            k_sync_approx<true><<<grid, kApproxThreads, smem, ctx->stream>>> (ctx->dbT.as<float>(), s.have.as<unsigned char>(), ld, int (n_out), int (n_starts),
                                                                             t.sorted.as<ApproxEntry>(), t.groups.as<int>(), t.n_groups, t.n_bits,
-                                                                            ctx->a_ud.as<float>(), ctx->a_cnt.as<int>());
+                                                                            s.a_ud.as<float>(), s.a_cnt.as<int>());
           }
         else
           {
             if (set_smem (ctx, k_sync_approx<false>, smem)) return 1;
             PROF (ctx);
-            k_sync_approx<false><<<grid, kApproxThreads, smem, ctx->stream>>> (ctx->dbT.as<float>(), ctx->have.as<unsigned char>(), ld, int (n_out), int (n_starts),
+            k_sync_approx<false><<<grid, kApproxThreads, smem, ctx->stream>>> (ctx->dbT.as<float>(), s.have.as<unsigned char>(), ld, int (n_out), int (n_starts),
                                                                              t.sorted.as<ApproxEntry>(), t.groups.as<int>(), t.n_groups, t.n_bits,
-                                                                             ctx->a_ud.as<float>(), ctx->a_cnt.as<int>());
+                                                                             s.a_ud.as<float>(), s.a_cnt.as<int>());
           }
         LAUNCH_CHECK ("k_sync_approx");
       }
     }
   {
     PROF (ctx);
-    k_sync_quality<<<unsigned ((n_starts * 4 + 255) / 256), 256, 0, ctx->stream>>> (ctx->a_ud.as<float>(), ctx->a_cnt.as<int>(), int (n_starts), t.n_bits,
-                                                                                norm_div, ctx->q.as<double>());
+    k_sync_quality<<<unsigned ((n_starts * 4 + 255) / 256), 256, 0, ctx->stream>>> (s.a_ud.as<float>(), s.a_cnt.as<int>(), int (n_starts), t.n_bits,
+                                                                                norm_div, s.q.as<double>());
     LAUNCH_CHECK ("k_sync_quality");
   }
   {
     const long long n = n_starts * 4;
     PROF (ctx);
-    k_local_mean<<<unsigned ((n + 255) / 256), 256, 0, ctx->stream>>> (ctx->q.as<double>(), n, ctx->scores.as<awm_search_score>());
+    k_local_mean<<<unsigned ((n + 255) / 256), 256, 0, ctx->stream>>> (s.q.as<double>(), n, s.scores.as<awm_search_score>());
     LAUNCH_CHECK ("k_local_mean");
   }
-  ctx->n_scores_dev = size_t (n_starts) * 4;
+  s.n_scores = size_t (n_starts) * 4;
+  CK (cudaEventRecord (s.done, ctx->stream));
   if (scores_out)
     {
-      CK (cudaMemcpyAsync (scores_out, ctx->scores.p, size_t (n_starts) * 4 * sizeof (awm_search_score), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (scores_out, s.scores.p, size_t (n_starts) * 4 * sizeof (awm_search_score), cudaMemcpyDeviceToHost, ctx->stream));
       CK (cudaStreamSynchronize (ctx->stream));
     }
+  return 0;
+}
+
+} // namespace
+
+int
+awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last,
+                 double water_delta, awm_search_score *scores_out, size_t max_scores, size_t *n_scores)
+{
+  /* searches still running on s_approx write a_mags: the search below waits for them */
+  for (auto& s : ctx->aslot)
+    if (s.done)
+      CK (cudaStreamWaitEvent (ctx->stream, s.done, 0));
+  return approx_launch (ctx, ctx->aslot[ctx->cur_aslot], key_slot, mode, wav_first, wav_last, water_delta, scores_out, max_scores, n_scores);
+}
+
+int
+awm_sync_approx_enqueue (awm_ctx *ctx, int slot, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta)
+{
+  if (slot < 0 || slot > 1)
+    return fail (ctx, "awm_sync_approx_enqueue: bad slot %d", slot);
+  /* the slot keeps a pointer to the bound PCM until it is used: a buffer of the context would be overwritten by the next bind or
+   * prefetch in the meantime */
+  const void *own[] = { ctx->pcm_own.p, ctx->pref[0].buf.p, ctx->pref[1].buf.p, ctx->staged.p, ctx->pcm_rs.p };
+  for (const void *b : own)
+    if (b && ctx->pcm == b)
+      return fail (ctx, "awm_sync_approx_enqueue: the bound PCM must be the caller's device memory, not a buffer of the context");
+  CK (cudaSetDevice (ctx->device));
+  if (!ctx->s_approx)
+    CK (cudaStreamCreateWithFlags (&ctx->s_approx, cudaStreamNonBlocking));
+  /* the PCM may have been written, and the slot's buffers may still be read, by work queued on the context stream */
+  cudaEvent_t busy;
+  CK (cudaEventCreateWithFlags (&busy, cudaEventDisableTiming));
+  CK (cudaEventRecord (busy, ctx->stream));
+  CK (cudaStreamWaitEvent (ctx->s_approx, busy, 0));
+  CK (cudaEventDestroy (busy));
+  /* the launch code queues its kernels and profiling records on ctx->stream */
+  cudaStream_t main_stream = ctx->stream;
+  ctx->stream = ctx->s_approx;
+  size_t n_scores = 0;
+  const int r = approx_launch (ctx, ctx->aslot[slot], key_slot, mode, wav_first, wav_last, water_delta, nullptr, 0, &n_scores);
+  ctx->stream = main_stream;
+  return r;
+}
+
+int
+awm_sync_use_slot (awm_ctx *ctx, int slot, size_t *n_scores)
+{
+  if (slot < 0 || slot > 1 || !ctx->aslot[slot].done)
+    return fail (ctx, "awm_sync_use_slot: nothing searched in slot %d", slot);
+  awm_ctx::ApproxSlot& s = ctx->aslot[slot];
+  CK (cudaSetDevice (ctx->device));
+  CK (cudaStreamWaitEvent (ctx->stream, s.done, 0));
+  ctx->cur_aslot = slot;
+  ctx->pcm = s.pcm;
+  ctx->pcm_frames = s.pcm_frames;
+  ctx->pcm_ch = s.pcm_ch;
+  if (n_scores)
+    *n_scores = s.n_scores;
   return 0;
 }
 
@@ -1588,7 +1684,8 @@ awm_sync_peaks (awm_ctx *ctx, double min_abs_quality, awm_search_score *out, siz
   if (!n || (max && !out))
     return fail (ctx, "awm_sync_peaks: bad arguments");
   *n = 0;
-  if (!ctx->n_scores_dev)
+  awm_ctx::ApproxSlot& s = ctx->aslot[ctx->cur_aslot];
+  if (!s.n_scores)
     return 0;
   CK (cudaSetDevice (ctx->device));
   /* counter and entries share one buffer ([u64 count, u64 pad][entries]) so that the usual case -- a few dozen peaks -- comes back
@@ -1597,9 +1694,9 @@ awm_sync_peaks (awm_ctx *ctx, double min_abs_quality, awm_search_score *out, siz
   CK (ctx->peaks_out.reserve (kHead + std::max<size_t> (max, 1) * sizeof (awm_search_score)));
   unsigned char *base = ctx->peaks_out.as<unsigned char>();
   CK (cudaMemsetAsync (base, 0, kHead, ctx->stream));
-  const long long ns = (long long) ctx->n_scores_dev;
+  const long long ns = (long long) s.n_scores;
   PROF (ctx);
-  k_peaks<<<unsigned ((ns + 255) / 256), 256, 0, ctx->stream>>> (ctx->scores.as<awm_search_score>(), ns, min_abs_quality,
+  k_peaks<<<unsigned ((ns + 255) / 256), 256, 0, ctx->stream>>> (s.scores.as<awm_search_score>(), ns, min_abs_quality,
                                                                 reinterpret_cast<awm_search_score *> (base + kHead), (unsigned long long) max,
                                                                 reinterpret_cast<unsigned long long *> (base));
   LAUNCH_CHECK ("k_peaks");
@@ -1628,10 +1725,12 @@ awm_sync_peaks (awm_ctx *ctx, double min_abs_quality, awm_search_score *out, siz
 }
 
 /* force: -1 = default kernel choice, 0 = sliding DFT, 1 = fresh FFT per offset.  With q_out the per-offset qualities of that
- * kernel are written ([n_scores][65], invalid offsets flagged 0 in valid_out) and the scores are left alone. */
+ * kernel are written ([n_scores][65], invalid offsets flagged 0 in valid_out) and the scores are left alone.  With rescored_out
+ * ([n_scores][65]) the sliding pass runs and the offsets k_refine_rank picks for exact re-scoring are flagged 1. */
 static int
 refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last,
-             double water_delta, awm_search_score *scores, size_t n_scores, int force, double *q_out, unsigned char *valid_out)
+             double water_delta, awm_search_score *scores, size_t n_scores, int force, double *q_out, unsigned char *valid_out,
+             unsigned char *rescored_out = nullptr)
 {
   if (key_slot < 0 || key_slot >= AWM_MAX_KEYS || mode < 0 || mode > 1 || (n_scores && !scores))
     return fail (ctx, "awm_sync_refine: bad arguments");
@@ -1669,6 +1768,8 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
     }
   CK (cudaMemcpyAsync (ctx->cand_start.p, h_start, nc * sizeof (long long), cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaMemcpyAsync (ctx->cand_noff.p, h_noff, nc * sizeof (int), cudaMemcpyHostToDevice, ctx->stream));
+  if (rescored_out)
+    force = 0;
   /* default: sliding DFT over the 65 offsets (awm_refine_slide.cuh); AWM_REFINE=fft selects the kernel that transforms every
    * frame of every offset afresh (also used for more than two channels) */
   static const bool force_fft = [] { const char *e = getenv ("AWM_REFINE"); return e && !strcmp (e, "fft"); } ();
@@ -1687,7 +1788,8 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
           CK (cudaMemcpy (ctx->tw1024.p, tw.data(), tw.size() * sizeof (float2), cudaMemcpyHostToDevice));
         }
       const size_t n_pairs = size_t (nc) * kOffsets * t.n_ent;
-      CK (ctx->r_ent_ud.reserve (n_pairs * sizeof (float2)));
+      /* also what the exact re-score of up to all 65 offsets stores there (k_refine_exact_fft_n): no reallocation between the kernels */
+      CK (ctx->r_ent_ud.reserve (std::max (n_pairs * sizeof (float2), n_pairs * 2 * kUD * sizeof (float))));
       CK (ctx->r_ent_flag.reserve (n_pairs));
       const size_t smem = fft_smem_bytes (kSlideWarps);
       const long long jobs = (long long) nc * t.n_ent;
@@ -1733,16 +1835,6 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
        * x 6 bits re-read them from L2 */
       prof_bytes (ctx, double (nc) * double (t.n_ent) * (double (kFrame) + 512.0) * ctx->pcm_ch * sizeof (float));
     }
-  const size_t n_ud = nc * kOffsets * n_bits * 2, n_cnt = nc * kOffsets * n_bits, n_val = nc * kOffsets;
-  float *h_ud = ctx->pin.get<float> (n_ud);
-  int *h_cnt = ctx->pin.get<int> (n_cnt);
-  unsigned char *h_valid = ctx->pin.get<unsigned char> (n_val);
-  if (!h_ud || !h_cnt || !h_valid)
-    return fail (ctx, "awm_sync_refine: out of page-locked memory");
-  CK (cudaMemcpyAsync (h_ud, ctx->r_ud.p, n_ud * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
-  CK (cudaMemcpyAsync (h_cnt, ctx->r_cnt.p, n_cnt * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-  CK (cudaMemcpyAsync (h_valid, ctx->rvalid.p, n_val, cudaMemcpyDeviceToHost, ctx->stream));
-  CK (cudaStreamSynchronize (ctx->stream));
   // sync_decode epilogue (src/syncfinder.cc:94-114,144-152) from the per-bit float sums
   auto quality_of = [&] (const float *ud, const int *cnt, size_t base) -> double
     {
@@ -1766,6 +1858,130 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
         sync_quality /= bit_count;
       return sync_quality / norm_div / 2.9;
     };
+  if (used_slide && !q_out)
+    {
+      /* The sliding DFT only RANKS the 65 offsets: every offset whose sliding score S lies within kVerifyMargin of the best sliding
+       * score is scored again with fresh FFTs in the reference's summation order (k_refine_exact_fft / _sum compute what k_refine
+       * computes), and the reference's rule picks among those exact values E.  If |S - E| <= d for all offsets, the exact arg-max o*
+       * satisfies S(o*) >= E(o*) - d >= E(o') - d >= S(o') - 2d for the sliding arg-max o', so with kVerifyMargin >= 2d the exact
+       * arg-max is always re-scored and index / quality are those of the exact kernel.  d is measured by
+       * tests/test_gpu_stages.py::test_sync_refine_vs_oracle (asserted < kVerifyMargin / 4 on all 65 offsets of every golden candidate); neighbouring offsets
+       * of a real peak differ by ~3e-3, so usually one or two offsets are re-scored.  The offset of the approx index itself is
+       * always re-scored: in the reference the search starts from the approx quality, which there IS the exact value of that
+       * offset (same transforms, same order of additions); ours comes from the entry-sum formulation and differs by ~1e-5
+       * relative, so the exact value takes its place below.  k_refine_rank picks the offsets on the device (the same rule as
+       * tests/test_gpu_refine_rank.py applies on the host), so the sliding sums never leave the GPU. */
+      constexpr double kVerifyMargin = 1e-3;
+      const size_t np_max = nc * kOffsets;
+      CK (ctx->cand_score.reserve (nc * sizeof (awm_search_score)));
+      CK (ctx->rank_keep.reserve (nc * 3 * sizeof (unsigned)));
+      CK (ctx->rank_first.reserve (nc * sizeof (int)));
+      CK (ctx->ex_start.reserve (np_max * sizeof (long long)));
+      CK (ctx->ex_cand.reserve (np_max * sizeof (int)));
+      CK (ctx->ex_off.reserve (np_max * sizeof (int)));
+      CK (ctx->ex_n.reserve (sizeof (int)));
+      awm_search_score *h_sc = ctx->pin.get<awm_search_score> (nc);
+      if (!h_sc)
+        return fail (ctx, "awm_sync_refine: out of page-locked memory");
+      std::copy (scores, scores + nc, h_sc);
+      CK (cudaMemcpyAsync (ctx->cand_score.p, h_sc, nc * sizeof (awm_search_score), cudaMemcpyHostToDevice, ctx->stream));
+      PROF (ctx);
+      k_refine_rank<<<1, kRankWarps * 32, 0, ctx->stream>>> (ctx->r_ud.as<float>(), ctx->r_cnt.as<int>(), ctx->rvalid.as<unsigned char>(),
+        ctx->cand_score.as<awm_search_score>(), ctx->cand_start.as<long long>(), ctx->cand_noff.as<int>(), int (nc), n_bits, norm_div, kVerifyMargin,
+        ctx->rank_keep.as<unsigned>(), ctx->rank_first.as<int>(), ctx->ex_start.as<long long>(), ctx->ex_cand.as<int>(), ctx->ex_off.as<int>(), ctx->ex_n.as<int>());
+      LAUNCH_CHECK ("k_refine_rank");
+      int *e_n = ctx->pin.get<int> (1);
+      int *e_cand = ctx->pin.get<int> (np_max);
+      int *e_off = ctx->pin.get<int> (np_max);
+      if (!e_n || !e_cand || !e_off)
+        return fail (ctx, "awm_sync_refine: out of page-locked memory");
+      if (rescored_out)
+        {
+          CK (cudaMemcpyAsync (e_n, ctx->ex_n.p, sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+          CK (cudaMemcpyAsync (e_cand, ctx->ex_cand.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+          CK (cudaMemcpyAsync (e_off, ctx->ex_off.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+          CK (cudaStreamSynchronize (ctx->stream));
+          std::fill (rescored_out, rescored_out + nc * kOffsets, 0);
+          for (int p = 0; p < *e_n; p++)
+            rescored_out[size_t (e_cand[p]) * kOffsets + e_off[p]] = 1;
+          return 0;
+        }
+      if (!ctx->n_sms)
+        CK (cudaDeviceGetAttribute (&ctx->n_sms, cudaDevAttrMultiProcessorCount, ctx->device));
+      const size_t smem = fft_smem_bytes (kExactWarps) + kExactWarps * 96 * sizeof (float);
+      if (set_smem (ctx, k_refine_exact_fft_n, smem)) return 1;
+      const long long jobs_max = (long long) np_max * t.n_ent;
+      PROF (ctx);
+      k_refine_exact_fft_n<<<unsigned (std::min<long long> ((jobs_max + kExactWarps - 1) / kExactWarps, 4LL * ctx->n_sms)), kExactWarps * 32, smem, ctx->stream>>> (
+        ctx->pcm, (long long) ctx->pcm_frames, ctx->pcm_ch, ctx->ex_start.as<long long>(), ctx->ex_n.as<int>(), t.ent.as<awm_sync_entry>(), t.n_ent,
+        ctx->r_ent_ud.as<float>(), ctx->tw.as<float2>(), ctx->win.as<float>());
+      LAUNCH_CHECK ("k_refine_exact_fft_n");
+      /* the re-scored offsets of a candidate lie within 512 samples of each other: its sync frames are compulsory traffic once
+       * (and were read by the sliding pass a moment ago: they come from L2) */
+      prof_bytes (ctx, double (nc) * double (t.n_ent) * (double (kFrame) + 512.0) * ctx->pcm_ch * sizeof (float));
+      int max_bit_frames = 1;
+      for (int b = 0; b < n_bits; b++)
+        max_bit_frames = std::max (max_bit_frames, t.h_off[b + 1] - t.h_off[b]);
+      const size_t sum_smem = size_t (kExactSumWarps) * max_bit_frames * kUD * sizeof (float);
+      if (set_smem (ctx, k_refine_exact_sum_n, sum_smem)) return 1;
+      const long long sum_jobs_max = (long long) np_max * n_bits * 2;
+      PROF (ctx);
+      k_refine_exact_sum_n<<<unsigned (std::min<long long> ((sum_jobs_max + kExactSumWarps - 1) / kExactSumWarps, 16LL * ctx->n_sms)), kExactSumWarps * 32, sum_smem, ctx->stream>>> (
+        ctx->r_ent_ud.as<float>(), ctx->ex_start.as<long long>(), ctx->ex_n.as<int>(), (long long) ctx->pcm_frames, ctx->pcm_ch, t.ent.as<awm_sync_entry>(), t.n_ent,
+        t.off.as<int>(), n_bits, total, (long long) wav_first, (long long) wav_last, max_bit_frames, ctx->r_ud.as<float>(), ctx->r_cnt.as<int>(), ctx->rvalid.as<unsigned char>());
+      LAUNCH_CHECK ("k_refine_exact_sum_n");
+      /* one round trip: the list, its length and the exact sums (sized for the longest list the rank can write) */
+      float *e_ud = ctx->pin.get<float> (np_max * n_bits * 2);
+      int *e_cnt = ctx->pin.get<int> (np_max * n_bits);
+      unsigned char *e_valid = ctx->pin.get<unsigned char> (np_max);
+      if (!e_ud || !e_cnt || !e_valid)
+        return fail (ctx, "awm_sync_refine: out of page-locked memory");
+      CK (cudaMemcpyAsync (e_n, ctx->ex_n.p, sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_cand, ctx->ex_cand.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_off, ctx->ex_off.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_ud, ctx->r_ud.p, np_max * n_bits * 2 * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_cnt, ctx->r_cnt.p, np_max * n_bits * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_valid, ctx->rvalid.p, np_max, cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaStreamSynchronize (ctx->stream));
+      const size_t np = size_t (*e_n);
+      std::vector<double> best_quality (nc);
+      std::vector<uint64_t> best_index (nc);
+      for (size_t c = 0; c < nc; c++)
+        {
+          best_quality[c] = scores[c].raw_quality;
+          best_index[c] = scores[c].index;
+        }
+      for (size_t p = 0; p < np; p++)               // starting value: the exact quality at the approx index
+        if (e_valid[p] && uint64_t (h_start[e_cand[p]] + 8LL * e_off[p]) == scores[e_cand[p]].index)
+          best_quality[e_cand[p]] = quality_of (e_ud, e_cnt, p);
+      for (size_t p = 0; p < np; p++)               // per candidate in ascending offset order
+        if (e_valid[p])
+          {
+            const size_t c = size_t (e_cand[p]);
+            const double q = quality_of (e_ud, e_cnt, p);
+            if (fabs (q - scores[c].local_mean) > fabs (best_quality[c] - scores[c].local_mean))   // src/syncfinder.cc:436-440
+              {
+                best_quality[c] = q;
+                best_index[c] = uint64_t (h_start[c] + 8LL * e_off[p]);
+              }
+          }
+      for (size_t c = 0; c < nc; c++)
+        {
+          scores[c].index = best_index[c];
+          scores[c].raw_quality = best_quality[c];
+        }
+      return 0;
+    }
+  const size_t n_ud = nc * kOffsets * n_bits * 2, n_cnt = nc * kOffsets * n_bits, n_val = nc * kOffsets;
+  float *h_ud = ctx->pin.get<float> (n_ud);
+  int *h_cnt = ctx->pin.get<int> (n_cnt);
+  unsigned char *h_valid = ctx->pin.get<unsigned char> (n_val);
+  if (!h_ud || !h_cnt || !h_valid)
+    return fail (ctx, "awm_sync_refine: out of page-locked memory");
+  CK (cudaMemcpyAsync (h_ud, ctx->r_ud.p, n_ud * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
+  CK (cudaMemcpyAsync (h_cnt, ctx->r_cnt.p, n_cnt * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+  CK (cudaMemcpyAsync (h_valid, ctx->rvalid.p, n_val, cudaMemcpyDeviceToHost, ctx->stream));
+  CK (cudaStreamSynchronize (ctx->stream));
   if (q_out)
     {
       for (size_t c = 0; c < nc; c++)
@@ -1775,115 +1991,6 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
             valid_out[c * kOffsets + o] = v ? 1 : 0;
             q_out[c * kOffsets + o] = v ? quality_of (h_ud, h_cnt, c * kOffsets + o) : 0.0;
           }
-      return 0;
-    }
-  if (used_slide)
-    {
-      /* The sliding DFT only RANKS the 65 offsets: every offset whose sliding score S lies within kVerifyMargin of the best sliding
-       * score is scored again with fresh FFTs in the reference's summation order (k_refine_exact_fft / _sum compute what k_refine
-       * computes), and the reference's rule picks among those exact values E.  If |S - E| <= d for all offsets, the exact arg-max o*
-       * satisfies S(o*) >= E(o*) - d >= E(o') - d >= S(o') - 2d for the sliding arg-max o', so with kVerifyMargin >= 2d the exact
-       * arg-max is always re-scored and index / quality are those of the exact kernel.  d is measured by
-       * tests/test_gpu_stages.py::test_sync_refine_vs_oracle (asserted < kVerifyMargin / 4 on all 65 offsets of every golden candidate); neighbouring offsets
-       * of a real peak differ by ~3e-3, so usually one or two offsets are re-scored. */
-      constexpr double kVerifyMargin = 1e-3;
-      std::vector<long long> p_start;
-      std::vector<int> p_noff, p_cand, p_off;
-      for (size_t c = 0; c < nc; c++)
-        {
-          std::vector<std::pair<double, int>> ranked;          // (-|q - local_mean|, offset): ascending sort = best first, lower offset first
-          for (int o = 0; o < h_noff[c]; o++)
-            if (h_valid[c * kOffsets + o])
-              ranked.push_back ({ -fabs (quality_of (h_ud, h_cnt, c * kOffsets + o) - scores[c].local_mean), o });
-          std::sort (ranked.begin(), ranked.end());
-          size_t keep = 0;
-          while (keep < ranked.size() && ranked[keep].first <= ranked[0].first + kVerifyMargin)
-            keep++;
-          ranked.resize (keep);
-          /* the offset of the approx index itself is always re-scored: in the reference the search starts from the approx quality,
-           * which there IS the exact value of that offset (same transforms, same order of additions); ours comes from the
-           * entry-sum formulation and differs by ~1e-5 relative, so the exact value takes its place below */
-          const int o_self = int (((long long) scores[c].index - h_start[c]) / 8);
-          if (o_self < h_noff[c] && h_valid[c * kOffsets + o_self]
-              && std::find_if (ranked.begin(), ranked.end(), [&] (const std::pair<double, int>& r) { return r.second == o_self; }) == ranked.end())
-            ranked.push_back ({ 0.0, o_self });
-          std::sort (ranked.begin(), ranked.end(), [] (const std::pair<double, int>& x, const std::pair<double, int>& y) { return x.second < y.second; });
-          for (const auto& r : ranked)
-            {
-              p_start.push_back (h_start[c] + 8LL * r.second);
-              p_noff.push_back (1);
-              p_cand.push_back (int (c));
-              p_off.push_back (r.second);
-            }
-        }
-      const size_t np = p_start.size();
-      float *e_ud = ctx->pin.get<float> (np * n_bits * 2);
-      int *e_cnt = ctx->pin.get<int> (np * n_bits);
-      unsigned char *e_valid = ctx->pin.get<unsigned char> (np);
-      long long *e_start = ctx->pin.get<long long> (np);
-      if (!e_ud || !e_cnt || !e_valid || !e_start)
-        return fail (ctx, "awm_sync_refine: out of page-locked memory");
-      std::copy (p_start.begin(), p_start.end(), e_start);
-      if (np)
-        {
-          CK (ctx->cand_start.reserve (np * sizeof (long long)));
-          CK (ctx->r_ent_ud.reserve (np * t.n_ent * 2 * kUD * sizeof (float)));
-          CK (ctx->r_ud.reserve (np * n_bits * 2 * sizeof (float)));
-          CK (ctx->r_cnt.reserve (np * n_bits * sizeof (int)));
-          CK (ctx->rvalid.reserve (np));
-          CK (cudaMemcpyAsync (ctx->cand_start.p, e_start, np * sizeof (long long), cudaMemcpyHostToDevice, ctx->stream));
-          const size_t smem = fft_smem_bytes (kExactWarps) + kExactWarps * 96 * sizeof (float);
-          if (set_smem (ctx, k_refine_exact_fft, smem)) return 1;
-          const long long jobs = (long long) np * t.n_ent;
-          PROF (ctx);
-          k_refine_exact_fft<<<unsigned ((jobs + kExactWarps - 1) / kExactWarps), kExactWarps * 32, smem, ctx->stream>>> (
-            ctx->pcm, (long long) ctx->pcm_frames, ctx->pcm_ch, ctx->cand_start.as<long long>(), int (np), t.ent.as<awm_sync_entry>(), t.n_ent,
-            ctx->r_ent_ud.as<float>(), ctx->tw.as<float2>(), ctx->win.as<float>());
-          LAUNCH_CHECK ("k_refine_exact_fft");
-          /* the re-scored offsets of a candidate lie within 512 samples of each other: its sync frames are compulsory traffic once
-           * (and were read by the sliding pass a moment ago: they come from L2) */
-          prof_bytes (ctx, double (nc) * double (t.n_ent) * (double (kFrame) + 512.0) * ctx->pcm_ch * sizeof (float));
-          PROF (ctx);
-          int max_bit_frames = 1;
-          for (int b = 0; b < n_bits; b++)
-            max_bit_frames = std::max (max_bit_frames, t.h_off[b + 1] - t.h_off[b]);
-          const size_t sum_smem = size_t (kExactSumWarps) * max_bit_frames * kUD * sizeof (float);
-          if (set_smem (ctx, k_refine_exact_sum, sum_smem)) return 1;
-          k_refine_exact_sum<<<unsigned ((np * n_bits * 2 + kExactSumWarps - 1) / kExactSumWarps), kExactSumWarps * 32, sum_smem, ctx->stream>>> (
-            ctx->r_ent_ud.as<float>(), ctx->cand_start.as<long long>(), int (np), (long long) ctx->pcm_frames, ctx->pcm_ch, t.ent.as<awm_sync_entry>(), t.n_ent,
-            t.off.as<int>(), n_bits, total, (long long) wav_first, (long long) wav_last, max_bit_frames, ctx->r_ud.as<float>(), ctx->r_cnt.as<int>(), ctx->rvalid.as<unsigned char>());
-          LAUNCH_CHECK ("k_refine_exact_sum");
-          CK (cudaMemcpyAsync (e_ud, ctx->r_ud.p, np * n_bits * 2 * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
-          CK (cudaMemcpyAsync (e_cnt, ctx->r_cnt.p, np * n_bits * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-          CK (cudaMemcpyAsync (e_valid, ctx->rvalid.p, np, cudaMemcpyDeviceToHost, ctx->stream));
-          CK (cudaStreamSynchronize (ctx->stream));
-        }
-      std::vector<double> best_quality (nc);
-      std::vector<uint64_t> best_index (nc);
-      for (size_t c = 0; c < nc; c++)
-        {
-          best_quality[c] = scores[c].raw_quality;
-          best_index[c] = scores[c].index;
-        }
-      for (size_t p = 0; p < np; p++)               // starting value: the exact quality at the approx index
-        if (e_valid[p] && uint64_t (p_start[p]) == scores[p_cand[p]].index)
-          best_quality[p_cand[p]] = quality_of (e_ud, e_cnt, p);
-      for (size_t p = 0; p < np; p++)               // per candidate in ascending offset order
-        if (e_valid[p])
-          {
-            const size_t c = size_t (p_cand[p]);
-            const double q = quality_of (e_ud, e_cnt, p);
-            if (fabs (q - scores[c].local_mean) > fabs (best_quality[c] - scores[c].local_mean))   // src/syncfinder.cc:436-440
-              {
-                best_quality[c] = q;
-                best_index[c] = uint64_t (h_start[c] + 8LL * p_off[p]);
-              }
-          }
-      for (size_t c = 0; c < nc; c++)
-        {
-          scores[c].index = best_index[c];
-          scores[c].raw_quality = best_quality[c];
-        }
       return 0;
     }
   for (size_t c = 0; c < nc; c++)
@@ -1915,6 +2022,16 @@ awm_sync_refine (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint6
                  double water_delta, awm_search_score *scores, size_t n_scores)
 {
   return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, scores, n_scores, -1, nullptr, nullptr);
+}
+
+int
+awm_sync_refine_rescored (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta,
+                          const awm_search_score *scores, size_t n_scores, unsigned char *rescored_out)
+{
+  if (!rescored_out)
+    return fail (ctx, "awm_sync_refine_rescored: bad arguments");
+  return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, const_cast<awm_search_score *> (scores), n_scores, 0,
+                      nullptr, nullptr, rescored_out);
 }
 
 int

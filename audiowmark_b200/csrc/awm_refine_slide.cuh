@@ -277,18 +277,12 @@ namespace awm {
 // k_refine_exact_sum adds the stored band values of a bit in the reference's order (frames ascending, 30 up / 30 down bands each).
 constexpr int kExactWarps = 8;
 
-__global__ void __launch_bounds__ (kExactWarps * 32, 2)
-k_refine_exact_fft (const float *__restrict__ pcm, long long n_frames, int C, const long long *__restrict__ pair_start, int n_pairs,
-                    const awm_sync_entry *__restrict__ g_ent, int n_ent, float *__restrict__ vals /* [pair][entry][60] */,
-                    const float2 *g_tw, const float *g_win)
+/* one (pair, sync frame) job of k_refine_exact_fft */
+__device__ __forceinline__ void
+refine_exact_fft_job (const float *__restrict__ pcm, long long n_frames, int C, const long long *__restrict__ pair_start,
+                      const awm_sync_entry *__restrict__ g_ent, int n_ent, float *__restrict__ vals, const FftSmem& s, float *sband,
+                      int lane, long long job)
 {
-  extern __shared__ __align__ (16) unsigned char smem[];
-  FftSmem s = fft_smem_setup (smem, g_tw, g_win, kExactWarps);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float *sband = s.extra + w * 96;
-  const long long job = (long long) blockIdx.x * kExactWarps + w;
-  if (job >= (long long) n_pairs * n_ent)
-    return;
   const int p = int (job / n_ent), e = int (job % n_ent);
   const awm_sync_entry *en = g_ent + e;
   const long long start = pair_start[p] + (long long) en->frame * kFrame;
@@ -304,23 +298,50 @@ k_refine_exact_fft (const float *__restrict__ pcm, long long n_frames, int C, co
     }
 }
 
+__global__ void __launch_bounds__ (kExactWarps * 32, 2)
+k_refine_exact_fft (const float *__restrict__ pcm, long long n_frames, int C, const long long *__restrict__ pair_start, int n_pairs,
+                    const awm_sync_entry *__restrict__ g_ent, int n_ent, float *__restrict__ vals /* [pair][entry][60] */,
+                    const float2 *g_tw, const float *g_win)
+{
+  extern __shared__ __align__ (16) unsigned char smem[];
+  FftSmem s = fft_smem_setup (smem, g_tw, g_win, kExactWarps);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  float *sband = s.extra + w * 96;
+  const long long job = (long long) blockIdx.x * kExactWarps + w;
+  if (job >= (long long) n_pairs * n_ent)
+    return;
+  refine_exact_fft_job (pcm, n_frames, C, pair_start, g_ent, n_ent, vals, s, sband, lane, job);
+}
+
+/* the same for a pair list whose length the device wrote (k_refine_rank): a fixed grid walks the jobs */
+__global__ void __launch_bounds__ (kExactWarps * 32, 2)
+k_refine_exact_fft_n (const float *__restrict__ pcm, long long n_frames, int C, const long long *__restrict__ pair_start, const int *__restrict__ n_pairs,
+                      const awm_sync_entry *__restrict__ g_ent, int n_ent, float *__restrict__ vals, const float2 *g_tw, const float *g_win)
+{
+  extern __shared__ __align__ (16) unsigned char smem[];
+  FftSmem s = fft_smem_setup (smem, g_tw, g_win, kExactWarps);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  float *sband = s.extra + w * 96;
+  const long long n_jobs = (long long) *n_pairs * n_ent;
+  for (long long job = (long long) blockIdx.x * kExactWarps + w; job < n_jobs; job += (long long) gridDim.x * kExactWarps)
+    {
+      __syncwarp();                               // the previous job's band values are read from sband
+      refine_exact_fft_job (pcm, n_frames, C, pair_start, g_ent, n_ent, vals, s, sband, lane, job);
+    }
+}
+
 // One warp per (pair, sync bit, up / down): the 30 band values of every frame of the bit are first staged in shared memory by the
 // whole warp (coalesced), then lane 0 adds them one after the other in the reference's order -- the chain of ~2550 dependent float
 // additions is what this kernel's time consists of, the loads no longer sit between them.
 constexpr int kExactSumWarps = 4;
 
-__global__ void __launch_bounds__ (kExactSumWarps * 32)
-k_refine_exact_sum (const float *__restrict__ vals, const long long *__restrict__ pair_start, int n_pairs, long long n_frames, int C,
-                    const awm_sync_entry *__restrict__ g_ent, int n_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,
-                    long long wav_first, long long wav_last, int max_bit_frames,
-                    float *__restrict__ out_ud /* [pair][n_bits][2] */, int *__restrict__ out_cnt, unsigned char *__restrict__ out_valid)
+/* one (pair, sync bit, up / down) job of k_refine_exact_sum */
+__device__ __forceinline__ void
+refine_exact_sum_job (const float *__restrict__ vals, const long long *__restrict__ pair_start, long long n_frames, int C,
+                      const awm_sync_entry *__restrict__ g_ent, int n_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,
+                      long long wav_first, long long wav_last, float *__restrict__ out_ud, int *__restrict__ out_cnt,
+                      unsigned char *__restrict__ out_valid, float *stage, int lane, int i)
 {
-  extern __shared__ __align__ (16) unsigned char smem[];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float *stage = reinterpret_cast<float *> (smem) + size_t (w) * max_bit_frames * kUD;
-  const int i = blockIdx.x * kExactSumWarps + w;
-  if (i >= n_pairs * n_bits * 2)
-    return;
   const int p = i / (n_bits * 2), bit = (i / 2) % n_bits, which = i & 1;       // which: 0 = up bands, 1 = down bands
   const long long fine = pair_start[p];
   const bool valid = fine + (long long) total_frame_count * kFrame <= n_frames;
@@ -351,6 +372,138 @@ k_refine_exact_sum (const float *__restrict__ vals, const long long *__restrict_
   out_ud[((size_t) p * n_bits + bit) * 2 + which] = mag;
   if (which == 0)
     out_cnt[(size_t) p * n_bits + bit] = cnt;
+}
+
+__global__ void __launch_bounds__ (kExactSumWarps * 32)
+k_refine_exact_sum (const float *__restrict__ vals, const long long *__restrict__ pair_start, int n_pairs, long long n_frames, int C,
+                    const awm_sync_entry *__restrict__ g_ent, int n_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,
+                    long long wav_first, long long wav_last, int max_bit_frames,
+                    float *__restrict__ out_ud /* [pair][n_bits][2] */, int *__restrict__ out_cnt, unsigned char *__restrict__ out_valid)
+{
+  extern __shared__ __align__ (16) unsigned char smem[];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  float *stage = reinterpret_cast<float *> (smem) + size_t (w) * max_bit_frames * kUD;
+  const int i = blockIdx.x * kExactSumWarps + w;
+  if (i >= n_pairs * n_bits * 2)
+    return;
+  refine_exact_sum_job (vals, pair_start, n_frames, C, g_ent, n_ent, g_bit_off, n_bits, total_frame_count, wav_first, wav_last,
+                        out_ud, out_cnt, out_valid, stage, lane, i);
+}
+
+/* the same for a pair list whose length the device wrote (k_refine_rank): a fixed grid walks the jobs */
+__global__ void __launch_bounds__ (kExactSumWarps * 32)
+k_refine_exact_sum_n (const float *__restrict__ vals, const long long *__restrict__ pair_start, const int *__restrict__ n_pairs, long long n_frames, int C,
+                      const awm_sync_entry *__restrict__ g_ent, int n_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,
+                      long long wav_first, long long wav_last, int max_bit_frames,
+                      float *__restrict__ out_ud, int *__restrict__ out_cnt, unsigned char *__restrict__ out_valid)
+{
+  extern __shared__ __align__ (16) unsigned char smem[];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  float *stage = reinterpret_cast<float *> (smem) + size_t (w) * max_bit_frames * kUD;
+  const int n_jobs = *n_pairs * n_bits * 2;
+  for (int i = blockIdx.x * kExactSumWarps + w; i < n_jobs; i += gridDim.x * kExactSumWarps)
+    {
+      __syncwarp();                               // lane 0 of the previous job has finished reading the stage
+      refine_exact_sum_job (vals, pair_start, n_frames, C, g_ent, n_ent, g_bit_off, n_bits, total_frame_count, wav_first, wav_last,
+                            out_ud, out_cnt, out_valid, stage, lane, i);
+    }
+}
+
+
+// ---- which offsets the exact kernels re-score --------------------------------------------------------------------------------
+// The rule of awm_sync_refine on the sums of k_refine_reduce, without a host round trip: per candidate the sync_decode quality of
+// every valid sliding offset (the host's quality_of, src/syncfinder.cc:94-114,144-152, in double and in the same order of
+// operations: float ratio, then the double products and sums unfused), every offset whose -|q - local_mean| lies within `margin`
+// of the smallest one, and the offset of the approx index if it is valid.  Output: the (start, candidate, offset) list in
+// candidate order, offsets ascending, and its length.  One CTA: warps own candidates, thread 0 places them one after the other.
+constexpr int kRankWarps = 32;
+
+__device__ __forceinline__ double
+rank_quality (const float *__restrict__ ud, const int *__restrict__ cnt, size_t base, int n_bits, double norm_div)
+{
+  double sync_quality = 0;
+  int bit_count = 0;
+  for (int bit = 0; bit < n_bits; bit++)
+    {
+      const size_t ob = base * n_bits + bit;
+      const float umag = ud[ob * 2], dmag = ud[ob * 2 + 1];
+      double raw_bit;
+      if (umag == 0 || dmag == 0)
+        raw_bit = 0;
+      else if (umag < dmag)
+        raw_bit = __fsub_rn (1.f, __fdiv_rn (umag, dmag));
+      else
+        raw_bit = __fsub_rn (__fdiv_rn (dmag, umag), 1.f);
+      sync_quality = __dadd_rn (sync_quality, __dmul_rn ((bit & 1) ? raw_bit : -raw_bit, double (cnt[ob])));
+      bit_count += cnt[ob];
+    }
+  if (bit_count)
+    sync_quality = __ddiv_rn (sync_quality, double (bit_count));
+  return __ddiv_rn (__ddiv_rn (sync_quality, norm_div), 2.9);
+}
+
+__global__ void __launch_bounds__ (kRankWarps * 32)
+k_refine_rank (const float *__restrict__ ud, const int *__restrict__ cnt, const unsigned char *__restrict__ valid,
+               const awm_search_score *__restrict__ cand, const long long *__restrict__ cand_start, const int *__restrict__ cand_noff,
+               int nc, int n_bits, double norm_div, double margin, unsigned *__restrict__ keep /* [nc][3] */, int *__restrict__ first /* [nc] */,
+               long long *__restrict__ out_start, int *__restrict__ out_cand, int *__restrict__ out_off, int *__restrict__ out_n)
+{
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int c = w; c < nc; c += kRankWarps)
+    {
+      double key[3];
+      bool ok[3];
+      double best = __longlong_as_double (0x7ff0000000000000LL);      // +inf
+      for (int k = 0; k < 3; k++)
+        {
+          const int o = lane + 32 * k;
+          ok[k] = o < cand_noff[c] && valid[(size_t) c * kOffsets + o];
+          key[k] = ok[k] ? -fabs (__dsub_rn (rank_quality (ud, cnt, (size_t) c * kOffsets + o, n_bits, norm_div), cand[c].local_mean)) : 0.0;
+          if (ok[k] && key[k] < best)
+            best = key[k];
+        }
+      for (int d = 16; d; d >>= 1)
+        best = fmin (best, __shfl_xor_sync (0xffffffffu, best, d));
+      const double limit = __dadd_rn (best, margin);
+      const int o_self = int (((long long) cand[c].index - cand_start[c]) / 8);
+      for (int k = 0; k < 3; k++)
+        {
+          const int o = lane + 32 * k;
+          const bool kept = ok[k] && (key[k] <= limit || o == o_self);
+          const unsigned m = __ballot_sync (0xffffffffu, kept);
+          if (lane == 0)
+            keep[c * 3 + k] = m;
+        }
+    }
+  __syncthreads();
+  if (threadIdx.x == 0)
+    {
+      int n = 0;
+      for (int c = 0; c < nc; c++)
+        {
+          first[c] = n;
+          n += __popc (keep[c * 3]) + __popc (keep[c * 3 + 1]) + __popc (keep[c * 3 + 2]);
+        }
+      *out_n = n;
+    }
+  __syncthreads();
+  for (int c = w; c < nc; c += kRankWarps)
+    {
+      int pos = first[c];
+      for (int k = 0; k < 3; k++)
+        {
+          const unsigned m = keep[c * 3 + k];
+          if (m >> lane & 1)
+            {
+              const int at = pos + __popc (m & ((1u << lane) - 1));
+              const int o = lane + 32 * k;
+              out_start[at] = cand_start[c] + 8LL * o;
+              out_cand[at] = c;
+              out_off[at] = o;
+            }
+          pos += __popc (m);
+        }
+    }
 }
 
 } // namespace awm

@@ -254,12 +254,12 @@ class BlockDecoder
 public:
   explicit BlockDecoder (double speed) : speed (speed) {}
 
-  /* the PCM (n_frames x n_channels at sample_rate) is already bound to the GPU context */
+  /* the PCM (n_frames x n_channels at sample_rate) is already bound to the GPU context, or searched in approx_slot (SyncFinder::search) */
   void
-  run (const vector<Key>& key_list, size_t n_frames, int n_channels, int sample_rate, vector<VitJob>& pending, int chunk)
+  run (const vector<Key>& key_list, size_t n_frames, int n_channels, int sample_rate, vector<VitJob>& pending, int chunk, int approx_slot = -1)
   {
     SyncFinder sync_finder;
-    key_results = sync_finder.search (key_list, n_frames, n_channels, SyncFinder::Mode::BLOCK, 0, n_frames * n_channels);
+    key_results = sync_finder.search (key_list, n_frames, n_channels, SyncFinder::Mode::BLOCK, 0, n_frames * n_channels, approx_slot);
     for (const auto& key_result : key_results)
       {
         const Key& key = key_result.key;
@@ -433,15 +433,16 @@ struct PcmRef
   }
 };
 
-/* decode (src/wmget.cc:886-939) for one chunk: everything up to the soft bits; the Viterbi jobs are queued */
+/* decode (src/wmget.cc:886-939) for one chunk: everything up to the soft bits; the Viterbi jobs are queued.
+ * approx_slot >= 0: one key, no speed detection; the chunk's approx search has been queued into that slot (awm_sync_approx_enqueue) */
 int
 decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vector<Key>& key_list, const PcmRef& pcm, size_t n_frames,
-              int n_channels, int sample_rate, bool first_chunk, bool print_speed_results = false)
+              int n_channels, int sample_rate, bool first_chunk, bool print_speed_results = false, int approx_slot = -1)
 {
   awm_ctx *ctx = Engine::ctx();
   if (!ctx)
     return 1;
-  if (pcm.bind (ctx, n_frames, n_channels))
+  if (approx_slot < 0 && pcm.bind (ctx, n_frames, n_channels))
     {
       error ("audiowmark: %s\n", awm_last_error (ctx));
       return 1;
@@ -503,7 +504,7 @@ decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vect
     }
   const double tb0 = get_time();
   BlockDecoder block_decoder (1);
-  block_decoder.run (key_list, n_frames, n_channels, sample_rate, pending, chunk);
+  block_decoder.run (key_list, n_frames, n_channels, sample_rate, pending, chunk, approx_slot);
   if (getenv ("AWM_TRACE"))
     fprintf (stderr, "[trace] chunk %d: block decoder (sync + soft bits) %.3f ms\n", chunk, (get_time() - tb0) * 1e3);
   if (first_chunk)
@@ -626,15 +627,40 @@ get_watermark_pcm (const vector<Key>& key_list, const float *samples, const int1
   pcm.f32 = samples16 ? nullptr : samples;
   pcm.s16 = samples16;
   pcm.prefetch (ctx, end - start, n_channels);
+  /* Device PCM of several chunks, one key, no speed detection: the approx search of chunk k + 1 is queued (on a second stream, into
+   * the other approx slot) before chunk k's candidate selection, refine and decode, so that the GPU has work while the host makes
+   * those decisions.  Every decision still runs per chunk, in the same order, on the same values.  Host PCM keeps the serial loop:
+   * there the next chunk's upload, not the GPU, sets the pace. */
+  const bool speed = Params::detect_speed || Params::detect_speed_patient || Params::try_speed > 0;
+  const int pipe_key = (!eof && key_list.size() == 1 && !speed && !Params::test_no_sync && pcm.f32 && Engine::is_device_pointer (pcm.f32))
+                       ? Engine::key_slot (key_list[0]) : -1;
+  auto enqueue_approx = [&] (size_t c0, size_t c1, int approx_slot)
+    {
+      if (pcm.advanced (c0 * n_channels).bind (ctx, c1 - c0, n_channels)
+          || awm_sync_approx_enqueue (ctx, approx_slot, pipe_key, AWM_MODE_BLOCK, 0, (c1 - c0) * n_channels, Params::water_delta))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return false;
+        }
+      return true;
+    };
+  if (pipe_key >= 0 && !enqueue_approx (start, end, 0))
+    return 1;
   for (;;)
     {
       string debug_sync;
+      const int chunk = int (time_offsets.size());
       if (!eof)
         {
           const size_t nstart = end - overlap, nend = min (nstart + max_frames, n_frames);
           pcm.advanced (nstart * n_channels).prefetch (ctx, nend - nstart, n_channels);
+          if (pipe_key >= 0 && !enqueue_approx (nstart, nend, (chunk + 1) & 1))
+            return 1;
+          if (pipe_key >= 0 && getenv ("AWM_TRACE"))
+            fprintf (stderr, "[trace] chunk %d: approx search of chunk %d queued ahead\n", chunk, chunk + 1);
         }
-      if (decode_chunk (pending, int (time_offsets.size()), debug_sync, key_list, pcm.advanced (start * n_channels), end - start, n_channels, sample_rate, first_chunk, print_speed_results))
+      if (decode_chunk (pending, chunk, debug_sync, key_list, pcm.advanced (start * n_channels), end - start, n_channels, sample_rate, first_chunk,
+                        print_speed_results, pipe_key >= 0 ? chunk & 1 : -1))
         return 1;
       time_offsets.push_back (time_offset);
       debug_syncs.push_back (debug_sync);

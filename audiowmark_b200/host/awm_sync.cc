@@ -252,7 +252,7 @@ SyncFinder::normalize_sync_quality (double raw_quality)
 }
 
 vector<SyncFinder::KeyResult>
-SyncFinder::search (const vector<Key>& key_list, size_t n_frames, int n_channels, Mode mode, size_t wav_first, size_t wav_last)
+SyncFinder::search (const vector<Key>& key_list, size_t n_frames, int n_channels, Mode mode, size_t wav_first, size_t wav_last, int approx_slot)
 {
   vector<KeyResult> key_results;
   awm_ctx *ctx = Engine::ctx();
@@ -296,7 +296,10 @@ SyncFinder::search (const vector<Key>& key_list, size_t n_frames, int n_channels
       if (ok)
         {
           size_t n_scores = 0;
-          ok = awm_sync_approx (ctx, slot, amode, wav_first, wav_last, Params::water_delta, nullptr, 0, &n_scores) == 0;
+          if (approx_slot >= 0)
+            ok = awm_sync_use_slot (ctx, approx_slot, &n_scores) == 0;
+          else
+            ok = awm_sync_approx (ctx, slot, amode, wav_first, wav_last, Params::water_delta, nullptr, 0, &n_scores) == 0;
           /* the scores stay on the device; normally only the peaks that matter come back */
           gpu_selected = ok && n_scores && select_candidates_gpu (ctx, Params::sync_threshold2 * 0.75, scores);
           if (gpu_selected)

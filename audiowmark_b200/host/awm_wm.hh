@@ -67,9 +67,10 @@ public:
   struct Score { size_t index; double quality; ConvBlockType block_type; };
   struct KeyResult { Key key; std::vector<Score> sync_scores; };
   /* searches the PCM currently bound to the GPU context; n_frames/n_channels describe it
-   * (padded length for CLIP mode), wav_first/wav_last = non-silent value range */
+   * (padded length for CLIP mode), wav_first/wav_last = non-silent value range.  approx_slot >= 0: one key, whose approx search
+   * has been queued with awm_sync_approx_enqueue into that slot (on the PCM to search, which need not be bound) */
   std::vector<KeyResult> search (const std::vector<Key>& key_list, size_t n_frames, int n_channels, Mode mode,
-                                 size_t wav_first, size_t wav_last);
+                                 size_t wav_first, size_t wav_last, int approx_slot = -1);
   static double normalize_sync_quality (double raw_quality);
 
   /* test aid: when tracing is on every search() call appends what it returns (mode, length of the searched signal and per key

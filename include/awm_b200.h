@@ -216,8 +216,17 @@ int awm_embed_batch_rates (awm_ctx *ctx, const void *in, void *out, int is_s16, 
 int awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last,
                      double water_delta, awm_search_score *scores_out, size_t max_scores, size_t *n_scores);
 
-/* awm_sync_peaks = sync_select_local_maxima (src/syncfinder.cc:258-281) on the score list of the last
- * awm_sync_approx call (kept on the device), restricted to peaks with |raw_quality - local_mean| > min_abs_quality:
+/* The search of awm_sync_approx without waiting for it: it is queued on a second stream of the context, behind everything queued on
+ * the context stream so far, and keeps its scores and its PCM view in approx slot `slot` (0 or 1), so that the search of the next
+ * chunk runs while the current chunk's peaks / refine / decode work on the other slot.  The bound PCM must stay valid (device
+ * memory of the caller) until the slot is used.  awm_sync_use_slot makes a slot current: the context stream waits for its search,
+ * the slot's PCM view becomes the bound PCM, awm_sync_peaks reads its scores; *n_scores as awm_sync_approx returns it.
+ * awm_sync_approx itself works on the current slot. */
+int awm_sync_approx_enqueue (awm_ctx *ctx, int slot, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta);
+int awm_sync_use_slot (awm_ctx *ctx, int slot, size_t *n_scores);
+
+/* awm_sync_peaks = sync_select_local_maxima (src/syncfinder.cc:258-281) on the score list of the current
+ * approx slot (kept on the device), restricted to peaks with |raw_quality - local_mean| > min_abs_quality:
  * only those can pass the threshold / n-best selection that follows, so the host never has to look at the
  * several hundred thousand scores of a 30 minute chunk.  out: sorted by index; *n = number found (may exceed max,
  * then only max entries were written and the caller should raise min_abs_quality or use awm_sync_approx's full list).
@@ -239,6 +248,12 @@ int awm_sync_refine (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, u
  * quality is within 1e-3 of the best exactly, so its result is that of the exact kernel as long as the two differ by < 5e-4. */
 int awm_sync_refine_offsets (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta,
                              const awm_search_score *scores, size_t n_scores, int exact, double *quality_out, unsigned char *valid_out);
+
+/* measurement aid for the parity tests: the fine offsets awm_sync_refine re-scores exactly, as its ranking kernel picks them on the
+ * device from the sliding qualities (every valid offset whose -|q - local_mean| is within 1e-3 of the smallest, plus the offset of the
+ * approx index if it is valid).  rescored_out: [n_scores][65], 1 = re-scored. */
+int awm_sync_refine_rescored (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta,
+                              const awm_search_score *scores, size_t n_scores, unsigned char *rescored_out);
 
 /* ---- block decode: FFTAnalyzer::fft_range (src/wmcommon.cc:123-141) + mix_decode
  * (src/wmget.cc:67-108) + randomize_bit_order(decode) for blocks starting at indices[i]
