@@ -1351,16 +1351,22 @@ batch_finish (awm_ctx *ctx, void *out_v, bool s16, size_t n_values, const float 
 }
 
 /* k_embed_batch work list entry of a non-empty item with awm_embed's geometry (limiter_block 0: no block peaks); advances the
- * launch's tile / limiter CTA counters and the flat peak array */
+ * launch's tile / limiter CTA counters and the flat peak array.  zero_frames: the item ends a stream that began that many
+ * sample-frames earlier with silence (awm_embed_batch_offsets); its processed range starts one frame before the item's first
+ * frame (awm_embed_batch.cuh) */
 BatchItem
-batch_entry (long long v0, long long n_frames, int C, int item, int limiter_block, long long& n_tiles, long long& n_lim, long long& n_peaks)
+batch_entry (long long v0, long long n_frames, int C, int item, int limiter_block, long long& n_tiles, long long& n_lim, long long& n_peaks,
+             long long zero_frames = 0)
 {
   BatchItem b;
   b.v0 = v0;
   b.n_frames = n_frames;
   b.C = C;
   b.item = item;
-  const long long n_proc = (b.n_frames + kFrame - 1) / kFrame + 1;
+  b.frame0 = zero_frames >= 2 * kFrame ? zero_frames / kFrame - 1 : 0;
+  b.lead = zero_frames - b.frame0 * kFrame;
+  b.blk0 = limiter_block > 0 ? b.frame0 * kFrame / limiter_block : 0;
+  const long long n_proc = (b.lead + b.n_frames + kFrame - 1) / kFrame + 1;
   b.tile0 = n_tiles;
   b.lim0 = n_lim;
   b.peak0 = n_peaks;
@@ -1375,13 +1381,14 @@ batch_entry (long long v0, long long n_frames, int C, int item, int limiter_bloc
  * Peaks go to ctx->peaks (zeroed by the caller), --snr sums to d_snr (null: none); delta_only: write the watermark signal alone */
 int
 launch_embed_batch (awm_ctx *ctx, const float *in, float *out, const BatchItem *d_items, int n_list, long long n_tiles, long long n_lim,
-                    int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling, double *d_snr, int delta_only)
+                    int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling, double *d_snr, int delta_only,
+                    bool offsets = false)
 {
   EmbedArgs A = {};
   A.in = in;
   A.out = out;
   A.fpb = ctx->roles_fpb;
-  A.frame_number0 = 2LL * A.fpb - frames_pad_start;       // first_frame_number 0: every item is a stream of its own
+  A.frame_number0 = 2LL * A.fpb - frames_pad_start;       // of a stream start; each item adds its frame0
   A.pow_up = 0.5f * float (-water_delta * 1);
   A.pow_down = 0.5f * float (-water_delta * -1);
   A.limiter_block = limiter_block;
@@ -1392,10 +1399,12 @@ launch_embed_batch (awm_ctx *ctx, const float *in, float *out, const BatchItem *
   A.tw = ctx->tw.as<float2>();
   A.win = ctx->win.as<float>();
   A.synth = ctx->synth.as<float>();
-  if (set_smem (ctx, k_embed_batch, kEmbedBatchSmem)) return 1;
+  /* items at stream offsets take their own instance: the offset arithmetic costs the stream-start case registers and spills */
+  auto kernel = offsets ? k_embed_batch<true> : k_embed_batch<false>;
+  if (set_smem (ctx, kernel, kEmbedBatchSmem)) return 1;
   PROF (ctx);
-  k_embed_batch<<<unsigned (n_tiles), kEmbedWarps * 32, kEmbedBatchSmem, ctx->stream>>> (A, d_items, n_list, ctx->roles.as<uint16_t>(),
-                                                                                        ctx->batch_coded.as<uint8_t>(), ctx->roles_n_coded);
+  kernel<<<unsigned (n_tiles), kEmbedWarps * 32, kEmbedBatchSmem, ctx->stream>>> (A, d_items, n_list, ctx->roles.as<uint16_t>(),
+                                                                                 ctx->batch_coded.as<uint8_t>(), ctx->roles_n_coded);
   LAUNCH_CHECK ("k_embed_batch");
   if (limiter_block > 0)
     {
@@ -1408,18 +1417,48 @@ launch_embed_batch (awm_ctx *ctx, const float *in, float *out, const BatchItem *
 
 } // namespace
 
+namespace {
+
+/* awm_batch_validate plus the offset list of awm_embed_batch_offsets (NULL: all zero) */
 int
-awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                 const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
-                 double *snr_power)
+batch_offsets_check (const awm_batch_item *items, size_t n_items, size_t n_values, const uint64_t *zero_frames, bool need_list, char *err, size_t err_cap)
+{
+  if (awm_batch_validate (items, n_items, n_values, err, err_cap))
+    return 1;
+  if (!zero_frames)
+    {
+      if (need_list && n_items)
+        {
+          if (err && err_cap)
+            snprintf (err, err_cap, "zero_frames list is NULL");
+          return 1;
+        }
+      return 0;
+    }
+  for (size_t i = 0; i < n_items; i++)
+    if (zero_frames[i] > AWM_MAX_STREAM_FRAMES || items[i].n_frames > AWM_MAX_STREAM_FRAMES - zero_frames[i])
+      {
+        if (err && err_cap)
+          snprintf (err, err_cap, "batch item %zu: zero_frames %llu + n_frames %llu exceeds the stream length limit of 2^48 frames", i,
+                    (unsigned long long) zero_frames[i], (unsigned long long) items[i].n_frames);
+        return 1;
+      }
+  return 0;
+}
+
+/* awm_embed_batch / awm_embed_batch_offsets (zero_frames NULL: every item starts a stream) */
+int
+embed_batch_any (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items,
+                 size_t n_items, const uint64_t *zero_frames, const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block,
+                 float limiter_ceiling, double *snr_power)
 {
   char why[160];
-  if (awm_batch_validate (items, n_items, n_values, why, sizeof (why)))
-    return fail (ctx, "awm_embed_batch: %s", why);
+  if (batch_offsets_check (items, n_items, n_values, zero_frames, false, why, sizeof (why)))
+    return fail (ctx, "%s: %s", name, why);
   if (!ctx->roles_fpb)
-    return fail (ctx, "awm_embed_batch: awm_set_embed_roles has not been called");
+    return fail (ctx, "%s: awm_set_embed_roles has not been called", name);
   if ((n_items && !coded_bits) || (n_values && (!in_v || !out_v)))
-    return fail (ctx, "awm_embed_batch: bad arguments");
+    return fail (ctx, "%s: bad arguments", name);
   if (snr_power)
     std::fill (snr_power, snr_power + 2 * n_items, 0.0);
   if (n_values == 0)
@@ -1440,10 +1479,10 @@ awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t
       covered += items[i].n_frames * uint64_t (items[i].channels);
       if (items[i].n_frames)
         list.push_back (batch_entry ((long long) items[i].value_offset, (long long) items[i].n_frames, items[i].channels, int (i), limiter_block,
-                                     n_tiles, n_lim, n_peaks));
+                                     n_tiles, n_lim, n_peaks, zero_frames ? (long long) zero_frames[i] : 0));
     }
   if (n_tiles >= INT_MAX || list.size() >= size_t (INT_MAX))
-    return fail (ctx, "awm_embed_batch: batch too large (%lld tiles)", n_tiles);
+    return fail (ctx, "%s: batch too large (%lld tiles)", name, n_tiles);
   if (covered < n_values)               /* values between items pass through unchanged */
     CK (cudaMemcpyAsync (d_out, d_in, n_values * sizeof (float), cudaMemcpyDeviceToDevice, ctx->stream));
   if (!list.empty())
@@ -1464,10 +1503,51 @@ awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t
           CK (cudaMemsetAsync (ctx->snr.p, 0, 2 * n_items * sizeof (double), ctx->stream));
         }
       if (launch_embed_batch (ctx, d_in, d_out, ctx->batch_items.as<BatchItem>(), int (list.size()), n_tiles, n_lim, frames_pad_start, water_delta,
-                              limiter_block, limiter_ceiling, snr_power ? ctx->snr.as<double>() : nullptr, 0))
+                              limiter_block, limiter_ceiling, snr_power ? ctx->snr.as<double>() : nullptr, 0, zero_frames != nullptr))
         return 1;
     }
   return batch_finish (ctx, out_v, s16, n_values, d_out, snr_power, list.empty() ? 0 : n_items);
+}
+
+} // namespace
+
+int
+awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                 const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
+                 double *snr_power)
+{
+  return embed_batch_any ("awm_embed_batch", ctx, in_v, out_v, is_s16, n_values, items, n_items, nullptr, coded_bits, frames_pad_start,
+                          water_delta, limiter_block, limiter_ceiling, snr_power);
+}
+
+int
+awm_batch_offsets_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const uint64_t *zero_frames, int sample_rate,
+                            int mark_sample_rate, char *err, size_t err_cap)
+{
+  if (batch_offsets_check (items, n_items, n_values, zero_frames, true, err, err_cap))
+    return 1;
+  if (sample_rate != mark_sample_rate)
+    for (size_t i = 0; i < n_items; i++)
+      if (zero_frames[i])
+        {
+          if (err && err_cap)
+            snprintf (err, err_cap, "batch item %zu: stream offsets are only supported at %d Hz", i, mark_sample_rate);
+          return 1;
+        }
+  if (err && err_cap)
+    err[0] = 0;
+  return 0;
+}
+
+int
+awm_embed_batch_offsets (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                         const uint64_t *zero_frames, const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block,
+                         float limiter_ceiling, double *snr_power)
+{
+  if (n_items && !zero_frames)
+    return fail (ctx, "awm_embed_batch_offsets: zero_frames list is NULL");
+  return embed_batch_any ("awm_embed_batch_offsets", ctx, in_v, out_v, is_s16, n_values, items, n_items, zero_frames, coded_bits, frames_pad_start,
+                          water_delta, limiter_block, limiter_ceiling, snr_power);
 }
 
 /* ---------------------------------------------------------------- sync search */

@@ -862,7 +862,8 @@ struct EmbedArgs
   unsigned *peaks;             // [n_blocks] float bits, atomicMax
   double *snr;                 // [2] or null
   long long snr_frames;        // frames that count for --snr (the reference loop stops earlier without limiter)
-  long long snr_pos0, snr_pos1; // ... and only positions [snr_pos0, snr_pos1) of this buffer (a window of a longer stream counts its own part)
+  long long snr_pos0, snr_pos1; // ... and only positions [snr_pos0, snr_pos1) of this buffer (a window of a longer stream counts its own part;
+                                //     embed_tile<.., LEAD>: in / out begin at snr_pos0)
   int delta_only;              // 1: write the watermark signal alone (WatermarkGen::run output), not input + watermark
   const float2 *tw;
   const float *win;
@@ -921,7 +922,11 @@ constexpr size_t kEmbedSmem = fft_smem_bytes (kEmbedWarps) + 3 * kFrame * sizeof
 // one CTA of k_embed: output frames [tile_first, tile_first + kEmbedTile) of the buffer A describes.  fm_row (r) returns the
 // 101-byte frame-mod row of table row r (0 keep, 1 up, 2 down); the whole warp calls it together.  VEC2: stereo in / out are
 // accessed as float2 (both 8-byte aligned); false uses single floats, with identical results.
-template<bool VEC2, class FmRow> __device__ __forceinline__ void
+// LEAD: in / out hold only the owned part [A.snr_pos0, A.n_frames) of the processed range, position p is their sample
+// p - A.snr_pos0 (a stream segment whose first frame begins in silence that is not in memory, k_embed_batch).  Positions before
+// the owned part read as zero without a load, are never written, and still count for the limiter block peaks.  LEAD = false is
+// k_embed's code unchanged.
+template<bool VEC2, bool LEAD = false, class FmRow> __device__ __forceinline__ void
 embed_tile (const EmbedArgs& A, long long tile_first, unsigned char *smem, FmRow fm_row)
 {
   FftSmem s = fft_smem_setup (smem, A.tw, A.win, kEmbedWarps);
@@ -954,7 +959,10 @@ embed_tile (const EmbedArgs& A, long long tile_first, unsigned char *smem, FmRow
       __syncthreads();                                      // synth[] ready / previous pair's edges consumed
       if (exists)
         {
-          load_pair<VEC2> (A.in, A.n_frames, C, m * kFrame, chA, chB, s.win, re, im, lane);
+          if constexpr (LEAD)                               // load_pair zeroes positions before in[0]
+            load_pair<VEC2> (A.in, A.n_frames - A.snr_pos0, C, m * kFrame - A.snr_pos0, chA, chB, s.win, re, im, lane);
+          else
+            load_pair<VEC2> (A.in, A.n_frames, C, m * kFrame, chA, chB, s.win, re, im, lane);
           fft1024_warp (re, im, s.tw, s.xbuf, lane);
           const long long r = (A.frame_number0 + m) % (2LL * A.fpb);
           const uint8_t *fm = fm_row (r);                   // rows [0,fpb) = A, [fpb,2fpb) = B
@@ -1016,7 +1024,25 @@ embed_tile (const EmbedArgs& A, long long tile_first, unsigned char *smem, FmRow
                 }
               const long long pos = m * kFrame + x;
               float oa = 0.f, ob = 0.f;
-              if (pos < A.n_frames)
+              if constexpr (LEAD)
+                {
+                  const long long q = pos - A.snr_pos0;             // index into in / out
+                  if (q >= 0 && pos < A.n_frames)
+                    {
+                      if (VEC2 && C == 2)
+                        {
+                          const float2 v = __ldg (reinterpret_cast<const float2 *> (A.in) + q);
+                          oa = v.x; ob = v.y;
+                        }
+                      else
+                        {
+                          oa = __ldg (A.in + q * C + chA);
+                          if (chB >= 0)
+                            ob = __ldg (A.in + q * C + chB);
+                        }
+                    }
+                }
+              else if (pos < A.n_frames)
                 {
                   if (VEC2 && C == 2)
                     {
@@ -1040,7 +1066,22 @@ embed_tile (const EmbedArgs& A, long long tile_first, unsigned char *smem, FmRow
               if (chB >= 0)
                 mx = fmaxf (mx, fabsf (yb));
               if (x < boundary) pk0 = fmaxf (pk0, mx); else pk1 = fmaxf (pk1, mx);
-              if (pos < A.n_frames)
+              if constexpr (LEAD)
+                {
+                  const long long q = pos - A.snr_pos0;
+                  if (q >= 0 && pos < A.n_frames)
+                    {
+                      if (VEC2 && C == 2)
+                        reinterpret_cast<float2 *> (A.out)[q] = make_float2 (ya, yb);
+                      else
+                        {
+                          A.out[q * C + chA] = ya;
+                          if (chB >= 0)
+                            A.out[q * C + chB] = yb;
+                        }
+                    }
+                }
+              else if (pos < A.n_frames)
                 {
                   if (VEC2 && C == 2)
                     reinterpret_cast<float2 *> (A.out)[pos] = make_float2 (ya, yb);
@@ -1097,10 +1138,11 @@ k_embed (EmbedArgs A)
 // ceiling / max (bm[b-1], bm[b]) and ceiling / max (bm[b], bm[b+1]); bm[b] = max (ceiling, peak[b]).
 constexpr int kLimiterIter = 16;        // sample-frames per thread: a CTA covers 4096 consecutive positions
 
-// one CTA of k_limiter: positions [cta_first, cta_first + blockDim.x * kLimiterIter) clipped to pos_end
+// one CTA of k_limiter: positions [cta_first, cta_first + blockDim.x * kLimiterIter) clipped to pos_end; position pos is
+// x[(pos - lead) * C ..] (lead > 0: the range starts in silence that is not in memory, see embed_tile)
 __device__ __forceinline__ void
 limiter_cta (float *__restrict__ x, long long cta_first, long long pos_end, int C, int block, float ceiling,
-             const unsigned *__restrict__ peaks, long long n_blocks, long long stream_pos0)
+             const unsigned *__restrict__ peaks, long long n_blocks, long long stream_pos0, long long lead = 0)
 {
   if (cta_first >= pos_end)
     return;
@@ -1135,7 +1177,7 @@ limiter_cta (float *__restrict__ x, long long cta_first, long long pos_end, int 
       const float scale_step = __fdiv_rn (__fsub_rn (scale_end, scale_start), float (block));
       const float scale = __fadd_rn (scale_start, __fmul_rn (float (i), scale_step));
       for (int c = 0; c < C; c++)
-        x[pos * C + c] = __fmul_rn (x[pos * C + c], scale);
+        x[(pos - lead) * C + c] = __fmul_rn (x[(pos - lead) * C + c], scale);
     }
 }
 

@@ -157,14 +157,19 @@ add_watermark_buffer_s16 (const Key& key, const int16_t *in, int16_t *out, size_
 
 int
 add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                     const vector<string>& bits, int sample_rate, vector<AddStats> *stats)
+                     const vector<string>& bits, int sample_rate, vector<AddStats> *stats, const uint64_t *zero_frames)
 {
+  char why[256];
+  if (zero_frames && awm_batch_offsets_validate (items, n_items, n_values, zero_frames, sample_rate, Params::mark_sample_rate, why, sizeof (why)))
+    {
+      error ("audiowmark: %s\n", why);
+      return 2;
+    }
   if (sample_rate != Params::mark_sample_rate)
     {
       error ("audiowmark: batched embedding is only available at %d Hz\n", Params::mark_sample_rate);
       return 2;
     }
-  char why[256];
   if (awm_batch_validate (items, n_items, n_values, why, sizeof (why)))
     {
       error ("audiowmark: %s\n", why);
@@ -184,8 +189,12 @@ add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t
     return 1;
   const int limiter_block = Params::test_no_limiter ? 0 : int (sample_rate * int (Params::limiter_block_size_ms) / 1000);
   vector<double> snr_power (2 * n_items);
-  if (awm_embed_batch (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), Params::frames_pad_start, Params::water_delta,
-                       limiter_block, Params::limiter_ceiling, (Params::snr || stats) ? snr_power.data() : nullptr))
+  const int rc = zero_frames
+    ? awm_embed_batch_offsets (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, zero_frames, coded.data(), Params::frames_pad_start,
+                               Params::water_delta, limiter_block, Params::limiter_ceiling, (Params::snr || stats) ? snr_power.data() : nullptr)
+    : awm_embed_batch (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), Params::frames_pad_start, Params::water_delta,
+                       limiter_block, Params::limiter_ceiling, (Params::snr || stats) ? snr_power.data() : nullptr);
+  if (rc)
     {
       error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
       return 1;
@@ -196,7 +205,9 @@ add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t
       const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
       for (size_t i = 0; i < n_items; i++)
         {
-          const size_t runs = gen_runs (items[i].n_frames, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000);
+          /* as add_watermark_windowed: the loop runs over the whole stream, silent prefix included */
+          const size_t n_stream = items[i].n_frames + (zero_frames ? zero_frames[i] : 0);
+          const size_t runs = gen_runs (n_stream, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000);
           const int blocks = int ((f0 + runs) / fpb - f0 / fpb);
           (*stats)[i].data_blocks = std::max (blocks - 1, 0);
           (*stats)[i].snr_db = snr_power[2 * i] > 0 ? 10 * log10 (snr_power[2 * i + 1] / snr_power[2 * i]) : INFINITY;

@@ -264,14 +264,14 @@ awmh_add (const unsigned char *key16, const float *in, float *out, size_t n_fram
  * data_blocks / snr_db (optional): [n_items].  Returns 2 for a malformed item list (checked before any GPU work). */
 static int
 add_batch_any (const unsigned char *key16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-               const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
+               const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db, const uint64_t *zero_frames = nullptr)
 {
   std::vector<std::string> bits (n_items);
   for (size_t i = 0; i < n_items; i++)
     bits[i] = payload_hex[i] ? payload_hex[i] : "";
   std::vector<AddStats> stats;
   const int rc = add_watermark_batch (make_key (key16, ""), in, out, s16, n_values, items, n_items, bits, sample_rate,
-                                      (data_blocks || snr_db) ? &stats : nullptr);
+                                      (data_blocks || snr_db) ? &stats : nullptr, zero_frames);
   for (size_t i = 0; i < stats.size(); i++)
     {
       if (data_blocks)
@@ -294,6 +294,23 @@ awmh_add_batch_s16 (const unsigned char *key16, const int16_t *in, int16_t *out,
                     const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
 {
   return add_batch_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db);
+}
+
+/* add_watermark_batch with stream offsets: items[i] continues a stream that began zero_frames[i] frames earlier with silence (an HLS
+ * segment; zero_frames NULL: all zero); otherwise as awmh_add_batch.  Returns 2 for a malformed offset list too
+ * (awm_batch_offsets_validate). */
+int
+awmh_add_batch_offsets (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                        const uint64_t *zero_frames, const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
+{
+  return add_batch_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db, zero_frames);
+}
+
+int
+awmh_add_batch_offsets_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                            const uint64_t *zero_frames, const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
+{
+  return add_batch_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db, zero_frames);
 }
 
 /* add_watermark_batch_rates on a packed buffer: items[i] is at sample_rates[i]; otherwise as awmh_add_batch */

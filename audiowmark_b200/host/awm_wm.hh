@@ -21,9 +21,11 @@ int add_watermark_buffer (const Key& key, const float *in, float *out, size_t n_
 
 /* add_watermark_buffer for many items of one packed buffer (float or 16 bit PCM, host or device), one payload per item, in one pass
  * over the GPU; item i comes out bit identical to add_watermark_buffer[_s16] on it alone.  44.1 kHz only.  stats (optional) gets
- * one entry per item.  Returns 2 for a malformed item list or payload, 1 for other errors. */
+ * one entry per item.  zero_frames (optional, [n_items]): item i continues a stream that began zero_frames[i] frames earlier with
+ * silence (HLS segments): it comes out as add_watermark_windowed with that zero_frames, its stats as that call reports them.
+ * Returns 2 for a malformed item list, offset list or payload, 1 for other errors. */
 int add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                         const std::vector<std::string>& bits, int sample_rate, std::vector<AddStats> *stats);
+                         const std::vector<std::string>& bits, int sample_rate, std::vector<AddStats> *stats, const uint64_t *zero_frames = nullptr);
 
 /* add_watermark_batch for items that each have their own sample rate (sample_rates[i]): item i comes out bit identical to
  * add_watermark_buffer on it alone at that rate (16 bit items: converted to float and back around it, as `audiowmark add` does for a

@@ -17,7 +17,8 @@ CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
            "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_add_windowed",
-           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16", "awmh_add_batch_rates", "awmh_add_batch_rates_s16"]
+           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16", "awmh_add_batch_rates", "awmh_add_batch_rates_s16",
+           "awmh_add_batch_offsets", "awmh_add_batch_offsets_s16"]
 
 _lib = None
 
@@ -218,24 +219,44 @@ def _pack_batch(name, pcms, payloads, items, out):
     return s16, it, n_values, p_in, p_out, split, (packed, res)
 
 
-def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False):
+def _zero_frames(name, zero_frames, n_items):
+    """a stream offset list -> uint64 array of n_items (ValueError for a wrong length or a value outside 0 .. 2^64-1)"""
+    z = list(zero_frames)
+    if len(z) != n_items:
+        raise ValueError("%s: %d items but %d zero_frames" % (name, n_items, len(z)))
+    if any(int(v) < 0 or int(v) >= 1 << 64 for v in z):
+        raise ValueError("%s: zero_frames must be in 0 .. 2^64-1" % name)
+    return np.array([int(v) for v in z], np.uint64)
+
+
+def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False, zero_frames=None):
     """`add` for many items with one key and one payload each, in one pass over the GPU; item i comes out bit identical to
     add / add_s16 of that item alone with payloads[i].
       pcms: a list of numpy arrays [n, channels] (all float32 or all int16; channels may differ), or one packed device tensor
             (float32 or int16, contiguous) with items = [(value_offset, n_frames, channels), ...] in values of that tensor;
             out: a device tensor like pcms for the result (default: a new one).
+      zero_frames: None, or one stream offset per item (sample-frames): item i continues a stream that began zero_frames[i]
+            frames earlier with silence, as an HLS segment does (`audiowmark hls-add`).  It comes out bit identical to
+            add_windowed(item, payloads[i], zero_frames=zero_frames[i]) = add(zeros(z) ++ item)[z:] (16 bit: add_s16 of the same),
+            with that call's data blocks and SNR.  zero_frames + n_frames is limited to 2^48 per item.
     Returns the list of outputs (numpy arrays, or views of the output tensor), with want_stats also the lists of data blocks
-    and SNR dB per item.  Only 44.1 kHz input is accepted.  Raises ValueError for a malformed item list or payload."""
+    and SNR dB per item.  Only 44.1 kHz input is accepted.  Raises ValueError for a malformed item list, offset list or payload."""
     payloads = list(payloads)
     s16, it, n_values, p_in, p_out, split, _keep = _pack_batch("add_batch", pcms, payloads, items, out)
+    z = None if zero_frames is None else _zero_frames("add_batch", zero_frames, len(it))
     pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
     blocks = np.zeros(max(len(it), 1), np.int32)
     snr = np.zeros(max(len(it), 1), np.float64)
-    fn = load().awmh_add_batch_s16 if s16 else load().awmh_add_batch
-    rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, ctypes.c_int(sample_rate),
-            _ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
+    stats = (_ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
+    if z is None:
+        fn = load().awmh_add_batch_s16 if s16 else load().awmh_add_batch
+        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, ctypes.c_int(sample_rate), *stats)
+    else:
+        fn = load().awmh_add_batch_offsets_s16 if s16 else load().awmh_add_batch_offsets
+        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), _ptr(z), pay, ctypes.c_int(sample_rate),
+                *stats)
     if rc == 2:
-        raise ValueError("add_batch: malformed item list or payload; see stderr")
+        raise ValueError("add_batch: malformed item list, offset list or payload; see stderr")
     if rc:
         raise RuntimeError("awmh_add_batch failed (rc=%d); see stderr" % rc)
     synchronize()

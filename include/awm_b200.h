@@ -188,6 +188,24 @@ int awm_batch_validate (const awm_batch_item *items, size_t n_items, size_t n_va
 int awm_embed_batch (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
                      const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
                      double *snr_power);
+/* Longest stream a batch item may end: zero_frames + n_frames <= 2^48 sample-frames (about 200 years at 44.1 kHz), so every stream
+ * position, limiter block boundary and interleaved value index of the embed kernels stays far inside their 64-bit arithmetic. */
+#define AWM_MAX_STREAM_FRAMES (1ull << 48)
+/* 0 if awm_batch_validate passes, zero_frames is not NULL (for n_items > 0), zero_frames[i] + n_frames of every item is at most
+ * AWM_MAX_STREAM_FRAMES and, when sample_rate != mark_sample_rate, every zero_frames[i] is 0; else nonzero with the reason in err.
+ * Needs no device. */
+int awm_batch_offsets_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const uint64_t *zero_frames, int sample_rate,
+                                int mark_sample_rate, char *err, size_t err_cap);
+/* awm_embed_batch for items that are segments of longer streams (HLS segments: add_stream_watermark with zero_frames,
+ * src/wmadd.cc:501-580).  Item i continues a stream that began zero_frames[i] sample-frames earlier with silence: it comes out bit
+ * identical to awm_embed (first_frame_number 0) of zeros (zero_frames[i]) ++ item, with the first zero_frames[i] frames dropped.
+ * Table rows, synthesis and limiter blocks are those of that stream; the silent prefix is never materialised, nothing outside an
+ * item's own values is read or written.  snr_power[i] sums the item's own positions only, as awm_embed_window does for the part
+ * it keeps.  zero_frames: [n_items], 44.1 kHz sample-frames; all zero gives exactly awm_embed_batch.  Everything else as
+ * awm_embed_batch. */
+int awm_embed_batch_offsets (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                             const uint64_t *zero_frames, const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block,
+                             float limiter_ceiling, double *snr_power);
 /* 0 if awm_batch_validate passes, mark_sample_rate > 0, every sample_rates[i] > 0, every rate other than mark_sample_rate has both
  * resampling ratios (mark / rate, rate / mark) inside the resampler's range (1/64, 64), at most 256 such rates are distinct and, where
  * n_emit is not NULL, n_emit[i] >= n_frames of every resampled item; else nonzero with the reason in err.  Needs no device. */
