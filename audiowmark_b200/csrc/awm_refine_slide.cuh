@@ -8,7 +8,8 @@
 //   Hann window  : the reference's window w[n] = (0.5 - 0.5 cos (2 pi n / 1024)) / 256 acts in the frequency domain as
 //                  X[k] = (R[k] - (R[k-1] + R[k+1]) / 2) / 512
 //   dB of bins 20..100 summed over the channels, up / down band sums of this sync frame (warp reduction)
-// ~290 warp instructions per offset instead of ~1700 for a fresh transform.  A second kernel adds the per-frame sums of each
+// The sample differences of all 64 slides are staged once in the warp's transpose buffer; the band sums of four offsets are
+// reduced together.  207 warp instructions per offset in stereo (117 mono) instead of ~1700 for a fresh transform.  A second kernel adds the per-frame sums of each
 // sync bit in frame order.  Numerics: a float sliding update carries an error of a few 1e-6 relative to the largest
 // bins after 64 steps, the same order as a float FFT's own rounding (DESIGN.md section 6); tests hold it to the
 // same bars as the FFT path (quality 2e-4, index within one 8-sample step).
@@ -20,6 +21,11 @@ namespace awm {
 
 constexpr int kSlideWarps = 8;
 constexpr int kSlideBins = 3;
+constexpr int kSlideGroup = 4;                          // offsets whose band sums are reduced together
+constexpr int kSlideStage = 8 * (kOffsets - 1);         // staged sample differences: 64 slides of 8
+constexpr float kSlideScale = 1.0f / 512.0f;            // the Hann window's 1/512, applied to the spectrum (exact: a power of two)
+constexpr float kSlideDbPerLog2 = 3.01029995663981f;    // 10 log10 (2): dB of |X|^2 = 10 log10 2 * log2 |X|^2
+constexpr float kSlideSilenceLog2 = -96.0f / kSlideDbPerLog2;
 
 template<int C> __global__ void __launch_bounds__ (kSlideWarps * 32, 2)
 k_refine_slide (const float *__restrict__ pcm, long long n_frames,
@@ -49,7 +55,7 @@ k_refine_slide (const float *__restrict__ pcm, long long n_frames,
   if (n_valid <= 0)
     return;
 
-  // ---- offset 0: rectangular-window spectrum by one FFT
+  // ---- offset 0: rectangular-window spectrum by one FFT, scaled by 1/512 (exact: a power of two)
   float rl_re[kSlideBins], rl_im[kSlideBins], rr_re[kSlideBins], rr_im[kSlideBins];
   {
     float re[32], im[32];
@@ -86,22 +92,57 @@ k_refine_slide (const float *__restrict__ pcm, long long n_frames,
       {
         const int k = (19 + kSlideBins * lane + b) & 127;
         const float4 v = sc[k];
-        rl_re[b] = v.x; rl_im[b] = v.y; rr_re[b] = v.z; rr_im[b] = v.w;
+        rl_re[b] = v.x * kSlideScale; rl_im[b] = v.y * kSlideScale; rr_re[b] = v.z * kSlideScale; rr_im[b] = v.w * kSlideScale;
       }
     __syncwarp();
   }
-  // ---- per-lane constants: W^(jk) for the 8 entering / leaving samples, the rotation W^(-8k), band membership
-  float wr[kSlideBins][8], wi[kSlideBins][8], rot_c[kSlideBins], rot_s[kSlideBins], m_up[kSlideBins], m_dn[kSlideBins];
+  if (n_valid > 1 && p0 + 8 * (n_valid - 2) + kFrame + 8 > n_frames)       // cannot happen (n_valid is cut to the stream above); keeps the loads in bounds
+    return;
+  // ---- the transpose buffer is free again: it takes the differences x[P + 1024 + n] - x[P + n] (scaled by 1/512 like the spectrum)
+  // of every slide, kSlideStage of them, zero past the last slide that exists.  Loaded once, coalesced; each slide then reads its 8
+  // (stereo: 8 x 2) as broadcast LDS.128 instead of every lane loading the same 16 samples from L2.
+  {
+    const int n_slide = int (8 * (n_valid - 1));
+    if (C == 2)
+      {
+        const float2 *po = reinterpret_cast<const float2 *> (pcm) + p0;
+        float2 *xb = reinterpret_cast<float2 *> (s.xbuf);
+#pragma unroll
+        for (int t = 0; t < kSlideStage / 32; t++)
+          {
+            const int i = 32 * t + lane;
+            float2 v = make_float2 (0.f, 0.f);
+            if (i < n_slide)
+              {
+                const float2 xo = __ldg (po + i), xi = __ldg (po + kFrame + i);
+                v = make_float2 ((xi.x - xo.x) * kSlideScale, (xi.y - xo.y) * kSlideScale);
+              }
+            xb[i] = v;
+          }
+      }
+    else
+      {
+#pragma unroll
+        for (int t = 0; t < kSlideStage / 32; t++)
+          {
+            const int i = 32 * t + lane;
+            s.xbuf[i] = i < n_slide ? (__ldg (pcm + p0 + kFrame + i) - __ldg (pcm + p0 + i)) * kSlideScale : 0.f;
+          }
+      }
+    __syncwarp();
+  }
+  // ---- per-lane constants: W^(jk) for the 7 entering / leaving samples j = 1..7 (W^0 = 1 is an add), the rotation W^(-8k), band membership
+  float wr[kSlideBins][7], wi[kSlideBins][7], rot_c[kSlideBins], rot_s[kSlideBins], m_up[kSlideBins], m_dn[kSlideBins];
 #pragma unroll
   for (int b = 0; b < kSlideBins; b++)
     {
       const int k = 19 + kSlideBins * lane + b;
 #pragma unroll
-      for (int j = 0; j < 8; j++)
+      for (int j = 1; j < 8; j++)
         {
           const float2 t = __ldg (tw1024 + ((j * k) & 1023));
-          wr[b][j] = t.x;
-          wi[b][j] = t.y;
+          wr[b][j - 1] = t.x;
+          wi[b][j - 1] = t.y;
         }
       const float2 r = __ldg (tw1024 + ((8 * k) & 1023));
       rot_c[b] = r.x;
@@ -118,46 +159,15 @@ k_refine_slide (const float *__restrict__ pcm, long long n_frames,
       m_dn[b] = md;
     }
 
-  // The 16 samples that enter / leave the frame at the next slide are loaded one iteration ahead: their latency hides behind the Hann /
-  // dB / reduction work of the current offset instead of stalling the first subtraction of the slide (17 % of this kernel's stall
-  // samples before).  The address is clamped to the last slide that exists, so the load itself needs no predicate.
-  auto load_delta = [&] (long long m, float (&dl)[8], float (&dr)[8])
+  // log2 |X|^2 for RANKING the offsets: MUFU.LG2 (abs. error ~1e-7 on these magnitudes -- an order below the float sliding DFT's own
+  // error) instead of the ~22-instruction log2f; the offsets that matter are scored again exactly by k_refine_exact_*.  A bin of
+  // exactly zero energy stands for -96 dB as in the reference.  The flush-to-zero MUFU alone is right for every normal energy; a lane
+  // that meets a zero or subnormal one takes the rule of __log2f (which scales subnormals first) on all six.  The band sums are
+  // turned into dB (x 10 log10 2) once, after the reduction.
+  auto lg_ftz = [] (float x) { float r; asm ("lg2.approx.ftz.f32 %0, %1;" : "=f" (r) : "f" (x)); return r; };
+  // per-lane part of the up / down band sums of the current spectrum: Hann in the frequency domain, log2 |X|^2 of both channels
+  auto band_partials = [&] (float& u, float& d)
     {
-      const long long mm = m + 1 < n_valid ? m : (n_valid >= 2 ? n_valid - 2 : 0);
-      const long long start = p0 + 8 * mm;
-      if (C == 2)
-        {
-          const float2 *po = reinterpret_cast<const float2 *> (pcm) + start;
-#pragma unroll
-          for (int j = 0; j < 8; j++)
-            {
-              const float2 xo = __ldg (po + j), xi = __ldg (po + kFrame + j);
-              dl[j] = xi.x - xo.x;
-              dr[j] = xi.y - xo.y;
-            }
-        }
-      else
-        {
-#pragma unroll
-          for (int j = 0; j < 8; j++)
-            {
-              dl[j] = __ldg (pcm + start + kFrame + j) - __ldg (pcm + start + j);
-              dr[j] = 0.f;
-            }
-        }
-    };
-  // dB for RANKING the offsets: MUFU.LG2 (__log2f, abs. error ~1e-7 on these magnitudes -- an order below the float sliding DFT's own
-  // error) instead of the ~22-instruction log2f; the offsets that matter are scored again exactly by k_refine_exact_*
-  auto db_fast = [] (float abs2) { return abs2 > 0.0f ? __log2f (abs2) * 3.01029995663981f : -96.0f; };
-  if (n_valid > 1 && p0 + 8 * (n_valid - 2) + kFrame + 8 > n_frames)       // cannot happen (n_valid is cut to the stream above); keeps the loads in bounds
-    return;
-  for (long long m = 0; m < n_valid; m++)
-    {
-      const long long start = p0 + 8 * m;
-      float dl[8], dr[8];
-      if (n_valid > 1)
-        load_delta (m, dl, dr);
-      // ---- Hann in the frequency domain + dB + band sums
       const float ll_re = __shfl_up_sync (0xffffffffu, rl_re[2], 1), ll_im = __shfl_up_sync (0xffffffffu, rl_im[2], 1);
       const float nl_re = __shfl_down_sync (0xffffffffu, rl_re[0], 1), nl_im = __shfl_down_sync (0xffffffffu, rl_im[0], 1);
       float lr_re = 0, lr_im = 0, nr_re = 0, nr_im = 0;
@@ -166,66 +176,155 @@ k_refine_slide (const float *__restrict__ pcm, long long n_frames,
           lr_re = __shfl_up_sync (0xffffffffu, rr_re[2], 1); lr_im = __shfl_up_sync (0xffffffffu, rr_im[2], 1);
           nr_re = __shfl_down_sync (0xffffffffu, rr_re[0], 1); nr_im = __shfl_down_sync (0xffffffffu, rr_im[0], 1);
         }
-      float u = 0.f, d = 0.f;
+      float e[C][kSlideBins];              // |X|^2 per channel and bin
 #pragma unroll
       for (int b = 0; b < kSlideBins; b++)
         {
           const float pl_re = b == 0 ? ll_re : rl_re[b - 1], pl_im = b == 0 ? ll_im : rl_im[b - 1];
           const float ql_re = b == kSlideBins - 1 ? nl_re : rl_re[b + 1], ql_im = b == kSlideBins - 1 ? nl_im : rl_im[b + 1];
           const float hl_re = rl_re[b] - 0.5f * (pl_re + ql_re), hl_im = rl_im[b] - 0.5f * (pl_im + ql_im);
-          // (1/512)^2 on the squared magnitude: exact power of two, same value as scaling the spectrum first
-          float db = db_fast ((hl_re * hl_re + hl_im * hl_im) * 3.814697265625e-06f);
+          e[0][b] = hl_re * hl_re + hl_im * hl_im;
           if (C == 2)
             {
               const float pr_re = b == 0 ? lr_re : rr_re[b - 1], pr_im = b == 0 ? lr_im : rr_im[b - 1];
               const float qr_re = b == kSlideBins - 1 ? nr_re : rr_re[b + 1], qr_im = b == kSlideBins - 1 ? nr_im : rr_im[b + 1];
               const float hr_re = rr_re[b] - 0.5f * (pr_re + qr_re), hr_im = rr_im[b] - 0.5f * (pr_im + qr_im);
-              db += db_fast ((hr_re * hr_re + hr_im * hr_im) * 3.814697265625e-06f);
+              e[C - 1][b] = hr_re * hr_re + hr_im * hr_im;
             }
-          u = fmaf (db, m_up[b], u);
-          d = fmaf (db, m_dn[b], d);
         }
+      float l2[C][kSlideBins], lo = e[0][0];
 #pragma unroll
-      for (int sh = 16; sh > 0; sh >>= 1)
+      for (int c = 0; c < C; c++)
+#pragma unroll
+        for (int b = 0; b < kSlideBins; b++)
+          {
+            l2[c][b] = lg_ftz (e[c][b]);
+            lo = fminf (lo, e[c][b]);
+          }
+      if (lo < 1.17549435e-38f)            // FLT_MIN
         {
-          u += __shfl_xor_sync (0xffffffffu, u, sh);
-          d += __shfl_xor_sync (0xffffffffu, d, sh);
+#pragma unroll
+          for (int c = 0; c < C; c++)
+#pragma unroll
+            for (int b = 0; b < kSlideBins; b++)
+              l2[c][b] = e[c][b] > 0.0f ? __log2f (e[c][b]) : kSlideSilenceLog2;
         }
-      if (lane == 0)
-        {
-          // frames in digital silence are not counted (src/syncfinder.cc:573-580)
-          const long long f_first = start * C, f_last = (start + kFrame) * C;
-          const bool counted = !(f_last < wav_first || f_first > wav_last);
-          out[(size_t) m * n_ent] = make_float2 (u, d);
-          flag[(size_t) m * n_ent] = counted ? 1 : 0;
-        }
-      if (m + 1 >= n_valid)
-        break;
-      // ---- slide by 8 samples
+      u = 0.f;
+      d = 0.f;
 #pragma unroll
       for (int b = 0; b < kSlideBins; b++)
         {
-          float tr = rl_re[b], ti = rl_im[b];
+          const float l = C == 2 ? l2[0][b] + l2[C - 1][b] : l2[0][b];
+          u = fmaf (l, m_up[b], u);
+          d = fmaf (l, m_dn[b], d);
+        }
+    };
+  // slide m: offset m -> m + 1, the 8 (stereo: 8 x 2) sample differences read from the stage as broadcast LDS.128
+  auto slide = [&] (int m)
+    {
+      float dl[8], dr[8];
+      if (C == 2)
+        {
+          const float4 *q = reinterpret_cast<const float4 *> (s.xbuf) + 4 * m;
 #pragma unroll
-          for (int j = 0; j < 8; j++)
+          for (int t = 0; t < 4; t++)
             {
-              tr = fmaf (dl[j], wr[b][j], tr);
-              ti = fmaf (dl[j], wi[b][j], ti);
+              const float4 v = q[t];
+              dl[2 * t] = v.x; dr[2 * t] = v.y; dl[2 * t + 1] = v.z; dr[2 * t + 1] = v.w;
+            }
+        }
+      else
+        {
+          const float4 *q = reinterpret_cast<const float4 *> (s.xbuf) + 2 * m;
+#pragma unroll
+          for (int t = 0; t < 2; t++)
+            {
+              const float4 v = q[t];
+              dl[4 * t] = v.x; dl[4 * t + 1] = v.y; dl[4 * t + 2] = v.z; dl[4 * t + 3] = v.w;
+              dr[4 * t] = dr[4 * t + 1] = dr[4 * t + 2] = dr[4 * t + 3] = 0.f;
+            }
+        }
+#pragma unroll
+      for (int b = 0; b < kSlideBins; b++)
+        {
+          float tr = rl_re[b] + dl[0], ti = rl_im[b];
+#pragma unroll
+          for (int j = 1; j < 8; j++)
+            {
+              tr = fmaf (dl[j], wr[b][j - 1], tr);
+              ti = fmaf (dl[j], wi[b][j - 1], ti);
             }
           rl_re[b] = tr * rot_c[b] - ti * rot_s[b];
           rl_im[b] = tr * rot_s[b] + ti * rot_c[b];
           if (C == 2)
             {
-              float sr = rr_re[b], si = rr_im[b];
+              float sr = rr_re[b] + dr[0], si = rr_im[b];
 #pragma unroll
-              for (int j = 0; j < 8; j++)
+              for (int j = 1; j < 8; j++)
                 {
-                  sr = fmaf (dr[j], wr[b][j], sr);
-                  si = fmaf (dr[j], wi[b][j], si);
+                  sr = fmaf (dr[j], wr[b][j - 1], sr);
+                  si = fmaf (dr[j], wi[b][j - 1], si);
                 }
               rr_re[b] = sr * rot_c[b] - si * rot_s[b];
               rr_im[b] = sr * rot_s[b] + si * rot_c[b];
             }
+        }
+    };
+  // frames in digital silence are not counted (src/syncfinder.cc:573-580)
+  auto counted = [&] (int m) -> unsigned char
+    {
+      const long long start = p0 + 8LL * m;
+      const long long f_first = start * C, f_last = (start + kFrame) * C;
+      return !(f_last < wav_first || f_first > wav_last);
+    };
+
+  // ---- offset 0
+  {
+    float u, d;
+    band_partials (u, d);
+#pragma unroll
+    for (int sh = 16; sh > 0; sh >>= 1)
+      {
+        u += __shfl_xor_sync (0xffffffffu, u, sh);
+        d += __shfl_xor_sync (0xffffffffu, d, sh);
+      }
+    if (lane == 0)
+      {
+        out[0] = make_float2 (u * kSlideDbPerLog2, d * kSlideDbPerLog2);
+        flag[0] = counted (0);
+      }
+  }
+  // ---- offsets 1..64 in groups of four.  The 8 per-lane partial sums of a group (u, d of each offset) are reduced together by a
+  // reduce-scatter: three halving exchanges (lanes 16, 8, 4 apart) leave lane l with value l >> 2 summed over 8 lanes, two butterflies
+  // finish it -- 10 shuffles per group instead of 10 per offset.  Lane 4g then holds u of offset m0 + g, lane 16 + 4g its d.
+  // Slides past the last valid offset read zero differences (the stage is zero there) and their sums are not stored.
+  static_assert (kSlideGroup == 4 && (kOffsets - 1) % kSlideGroup == 0, "the reduce-scatter below is written for groups of four");
+  for (int m0 = 1; m0 < n_valid; m0 += kSlideGroup)
+    {
+      float v[2 * kSlideGroup];
+#pragma unroll
+      for (int g = 0; g < kSlideGroup; g++)
+        {
+          slide (m0 + g - 1);
+          band_partials (v[g], v[kSlideGroup + g]);
+        }
+      const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4;
+      float a[4], b[2];
+#pragma unroll
+      for (int i = 0; i < 4; i++)
+        a[i] = (h16 ? v[i + 4] : v[i]) + __shfl_xor_sync (0xffffffffu, h16 ? v[i] : v[i + 4], 16);
+#pragma unroll
+      for (int i = 0; i < 2; i++)
+        b[i] = (h8 ? a[i + 2] : a[i]) + __shfl_xor_sync (0xffffffffu, h8 ? a[i] : a[i + 2], 8);
+      float r = (h4 ? b[1] : b[0]) + __shfl_xor_sync (0xffffffffu, h4 ? b[0] : b[1], 4);
+      r += __shfl_xor_sync (0xffffffffu, r, 2);
+      r += __shfl_xor_sync (0xffffffffu, r, 1);
+      const int g = (lane >> 2) & 3, m = m0 + g;
+      if ((lane & 3) == 0 && m < n_valid)
+        {
+          reinterpret_cast<float *> (out + (size_t) m * n_ent)[lane >> 4] = r * kSlideDbPerLog2;
+          if (lane < 16)
+            flag[(size_t) m * n_ent] = counted (m);
         }
     }
 }
