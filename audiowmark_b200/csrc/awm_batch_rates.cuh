@@ -1,11 +1,11 @@
-// awm_batch_rates.cuh -- batched embed of items at any sample rate (awm_embed_batch_rates in awm_capi.cu): the resampling steps of
-// awm_embed_resampled for many items of one packed buffer, each at its own rate, with one launch per step.
+// awm_batch_rates.cuh -- batched embed of items at any sample rate (awm_embed_batch_rates in awm_capi.cu): the add loop with a
+// WatermarkResampler (src/wmadd.cc:353-430, 548-566) for many items of one packed buffer, each at its own rate, with one launch per step.
 //
-//   k_resample_batch      in-resampler: item PCM -> the item at the watermark rate (scratch, zero extended: n_stop "never")
-//   (k_embed_batch)       WatermarkGen::run on it, delta_only: the watermark signal alone (scratch)
-//   k_resample_mix_batch  out-resampler fused with the mixer: for every frame the add loop emits, the watermark resampled back to
-//                         the item's rate + the input, the item's limiter block peaks and --snr sums (k_resample + k_mix_peaks
-//                         without the watermark buffer at the input rate in between)
+//   k_resample_batch      in-resampler (:392-393): item PCM -> the item at the watermark rate (scratch, zero extended as the loop
+//                         keeps feeding zero frames: n_stop "never")
+//   (k_embed_batch)       WatermarkGen::run on it (:394-399), delta_only: the watermark signal alone (scratch)
+//   k_resample_mix_batch  out-resampler (:401-406) fused with the mixer (:548-566): for every frame the add loop emits, the watermark
+//                         resampled back to the item's rate + the input, the item's limiter block peaks and --snr sums
 //   k_limiter_rates       k_limiter per item with the item's own block size
 //
 // Work lists as in k_embed_batch: all CTAs of a launch cost the same (256 output frames of one resampling job, 4096 limiter
@@ -92,7 +92,8 @@ k_resample_batch (const RateItem *__restrict__ items, int n_items)
 }
 
 // frame i < n_emit of an item: y = wm + orig (orig is zero beyond n_frames), stored for i < n_frames; peak of |y| per limiter block
-// of the item (only peaks above the ceiling matter); --snr sums of wm and orig.  The operations of k_resample + k_mix_peaks.
+// of the item (only peaks above the ceiling matter, Limiter::block_max starts at the ceiling); --snr sums of wm and orig.  The
+// watermark is resampled by the operations of k_resample and stays in registers.
 __global__ void __launch_bounds__ (kRateCta)
 k_resample_mix_batch (const RateItem *__restrict__ items, int n_items, float ceiling, unsigned *__restrict__ peaks, double *__restrict__ snr)
 {

@@ -1415,10 +1415,6 @@ launch_embed_batch (awm_ctx *ctx, const float *in, float *out, const BatchItem *
   return 0;
 }
 
-} // namespace
-
-namespace {
-
 /* awm_batch_validate plus the offset list of awm_embed_batch_offsets (NULL: all zero) */
 int
 batch_offsets_check (const awm_batch_item *items, size_t n_items, size_t n_values, const uint64_t *zero_frames, bool need_list, char *err, size_t err_cap)
@@ -1446,79 +1442,7 @@ batch_offsets_check (const awm_batch_item *items, size_t n_items, size_t n_value
   return 0;
 }
 
-/* awm_embed_batch / awm_embed_batch_offsets (zero_frames NULL: every item starts a stream) */
-int
-embed_batch_any (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items,
-                 size_t n_items, const uint64_t *zero_frames, const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block,
-                 float limiter_ceiling, double *snr_power)
-{
-  char why[160];
-  if (batch_offsets_check (items, n_items, n_values, zero_frames, false, why, sizeof (why)))
-    return fail (ctx, "%s: %s", name, why);
-  if (!ctx->roles_fpb)
-    return fail (ctx, "%s: awm_set_embed_roles has not been called", name);
-  if ((n_items && !coded_bits) || (n_values && (!in_v || !out_v)))
-    return fail (ctx, "%s: bad arguments", name);
-  if (snr_power)
-    std::fill (snr_power, snr_power + 2 * n_items, 0.0);
-  if (n_values == 0)
-    return 0;
-  CK (cudaSetDevice (ctx->device));
-  const bool s16 = is_s16 != 0;
-  const float *d_in;
-  float *d_out;
-  if (batch_images (ctx, in_v, out_v, s16, n_values, &d_in, &d_out))
-    return 1;
-
-  /* work list: non-empty items with their first tile, first limiter CTA and block peaks */
-  std::vector<BatchItem> list;
-  long long n_tiles = 0, n_lim = 0, n_peaks = 0;
-  uint64_t covered = 0;
-  for (size_t i = 0; i < n_items; i++)
-    {
-      covered += items[i].n_frames * uint64_t (items[i].channels);
-      if (items[i].n_frames)
-        list.push_back (batch_entry ((long long) items[i].value_offset, (long long) items[i].n_frames, items[i].channels, int (i), limiter_block,
-                                     n_tiles, n_lim, n_peaks, zero_frames ? (long long) zero_frames[i] : 0));
-    }
-  if (n_tiles >= INT_MAX || list.size() >= size_t (INT_MAX))
-    return fail (ctx, "%s: batch too large (%lld tiles)", name, n_tiles);
-  if (covered < n_values)               /* values between items pass through unchanged */
-    CK (cudaMemcpyAsync (d_out, d_in, n_values * sizeof (float), cudaMemcpyDeviceToDevice, ctx->stream));
-  if (!list.empty())
-    {
-      const size_t coded_bytes = n_items * 2 * size_t (ctx->roles_n_coded);
-      CK (ctx->batch_items.reserve (list.size() * sizeof (BatchItem)));
-      CK (ctx->batch_coded.reserve (coded_bytes));
-      CK (cudaMemcpyAsync (ctx->batch_items.p, list.data(), list.size() * sizeof (BatchItem), cudaMemcpyHostToDevice, ctx->stream));
-      CK (cudaMemcpyAsync (ctx->batch_coded.p, coded_bits, coded_bytes, cudaMemcpyHostToDevice, ctx->stream));
-      if (n_peaks)
-        {
-          CK (ctx->peaks.reserve (n_peaks * sizeof (unsigned)));
-          CK (cudaMemsetAsync (ctx->peaks.p, 0, n_peaks * sizeof (unsigned), ctx->stream));
-        }
-      if (snr_power)
-        {
-          CK (ctx->snr.reserve (2 * n_items * sizeof (double)));
-          CK (cudaMemsetAsync (ctx->snr.p, 0, 2 * n_items * sizeof (double), ctx->stream));
-        }
-      if (launch_embed_batch (ctx, d_in, d_out, ctx->batch_items.as<BatchItem>(), int (list.size()), n_tiles, n_lim, frames_pad_start, water_delta,
-                              limiter_block, limiter_ceiling, snr_power ? ctx->snr.as<double>() : nullptr, 0, zero_frames != nullptr))
-        return 1;
-    }
-  return batch_finish (ctx, out_v, s16, n_values, d_out, snr_power, list.empty() ? 0 : n_items);
-}
-
 } // namespace
-
-int
-awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                 const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
-                 double *snr_power)
-{
-  return embed_batch_any ("awm_embed_batch", ctx, in_v, out_v, is_s16, n_values, items, n_items, nullptr, coded_bits, frames_pad_start,
-                          water_delta, limiter_block, limiter_ceiling, snr_power);
-}
 
 int
 awm_batch_offsets_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const uint64_t *zero_frames, int sample_rate,
@@ -1537,17 +1461,6 @@ awm_batch_offsets_validate (const awm_batch_item *items, size_t n_items, size_t 
   if (err && err_cap)
     err[0] = 0;
   return 0;
-}
-
-int
-awm_embed_batch_offsets (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                         const uint64_t *zero_frames, const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block,
-                         float limiter_ceiling, double *snr_power)
-{
-  if (n_items && !zero_frames)
-    return fail (ctx, "awm_embed_batch_offsets: zero_frames list is NULL");
-  return embed_batch_any ("awm_embed_batch_offsets", ctx, in_v, out_v, is_s16, n_values, items, n_items, zero_frames, coded_bits, frames_pad_start,
-                          water_delta, limiter_block, limiter_ceiling, snr_power);
 }
 
 /* ---------------------------------------------------------------- sync search */
@@ -2512,8 +2425,8 @@ coef_table (awm_ctx *ctx, double ratio, int hlen, const float **coef, int *h_out
   return 0;
 }
 
-/* frames at the watermark rate an item of awm_embed_resampled needs: up to the highest tap of output n_emit - 1 (> 0), in whole
- * 1024-frames */
+/* frames at the watermark rate a resampled item of awm_embed_batch_rates needs: up to the highest tap of output n_emit - 1 (> 0), in
+ * whole 1024-frames */
 long long
 resampled_n44 (uint64_t n_emit, double step_out, int h_out)
 {
@@ -2670,128 +2583,7 @@ awm_copy_to_host (awm_ctx *ctx, void *dst, const void *src, size_t bytes)
   return 0;
 }
 
-/* ---------------------------------------------------------------- embed at other sample rates */
-
-int
-awm_embed_resampled (awm_ctx *ctx, const float *in, float *out, size_t n_frames, int channels, int sample_rate, int mark_sample_rate,
-                     size_t n_emit, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling, double *snr_power)
-{
-  if (!ctx->embed_fpb)
-    return fail (ctx, "awm_embed_resampled: awm_set_embed_tables has not been called");
-  if (channels <= 0 || sample_rate <= 0 || mark_sample_rate <= 0 || sample_rate == mark_sample_rate || n_emit < n_frames || (n_frames && (!in || !out)))
-    return fail (ctx, "awm_embed_resampled: bad arguments");
-  if (snr_power)
-    snr_power[0] = snr_power[1] = 0;
-  if (n_frames == 0)
-    return 0;
-  CK (cudaSetDevice (ctx->device));
-  const double r_in = double (mark_sample_rate) / sample_rate, r_out = double (sample_rate) / mark_sample_rate;
-  const float *coef_in, *coef_out;
-  int h_in, h_out;
-  if (coef_table (ctx, r_in, 16, &coef_in, &h_in) || coef_table (ctx, r_out, 16, &coef_out, &h_out))
-    return 1;
-  /* watermark frames needed for the emitted output: highest tap of output n_emit - 1 */
-  const double step_out = 1.0 / r_out;
-  const long long n44 = resampled_n44 (n_emit, step_out, h_out), n_blocks44 = n44 / kFrame;
-  const size_t n_val = n_frames * channels;
-  const bool in_dev = is_device_ptr (in), out_dev = is_device_ptr (out);
-  const float *d_in = in;
-  float *d_out = out;
-  if (!in_dev)
-    {
-      CK (ctx->emb_in.reserve (n_val * sizeof (float)));
-      CK (cudaMemcpyAsync (ctx->emb_in.p, in, n_val * sizeof (float), cudaMemcpyHostToDevice, ctx->stream));
-      d_in = ctx->emb_in.as<float>();
-    }
-  if (!out_dev)
-    {
-      CK (ctx->emb_out.reserve (n_val * sizeof (float)));
-      d_out = ctx->emb_out.as<float>();
-    }
-  CK (ctx->rs_in.reserve (size_t (n44) * channels * sizeof (float)));       /* x44: input at the watermark rate */
-  CK (ctx->rs_out.reserve (size_t (n44) * channels * sizeof (float)));      /* wm44: watermark signal at the watermark rate */
-  CK (ctx->pcm_rs.reserve (n_emit * channels * sizeof (float)));            /* watermark at the input rate */
-  ctx->pushed = false;
-  ctx->pcm_ch = ctx->pcm == ctx->pcm_rs.p ? 0 : ctx->pcm_ch;                 /* a pushed binding lived in pcm_rs */
-  /* 1. in_resampler (src/wmadd.cc:392-393): the loop keeps feeding zero frames, so the input is zero extended */
-  ResampleJob J;
-  J.in = d_in; J.out = ctx->rs_in.as<float>(); J.n_in = (long long) n_frames; J.n_stop = LLONG_MAX / 4; J.n_out = n44;
-  J.step = 1.0 / r_in; J.h = h_in; J.coef = coef_in;
-  if (launch_resample (ctx, { J }, channels))
-    return 1;
-  /* 2. WatermarkGen::run on every 1024-frame of it (src/wmadd.cc:394-399) */
-  {
-    EmbedArgs A;
-    A.in = ctx->rs_in.as<float>();
-    A.out = ctx->rs_out.as<float>();
-    A.n_frames = n44;
-    A.C = channels;
-    A.n_proc = n_blocks44 + 1;
-    A.frame_begin = 0;
-    A.frame_end = A.n_proc;
-    A.fpb = ctx->embed_fpb;
-    A.frame_number0 = 2LL * A.fpb - frames_pad_start;
-    A.frame_mod = ctx->frame_mod.as<uint8_t>();
-    A.pow_up = 0.5f * float (-water_delta * 1);
-    A.pow_down = 0.5f * float (-water_delta * -1);
-    A.limiter_block = 0;
-    A.stream_pos0 = 0;
-    A.blk0 = 0;
-    A.peaks = nullptr;
-    A.snr = nullptr;
-    A.snr_frames = 0;
-    A.snr_pos0 = 0;
-    A.snr_pos1 = LLONG_MAX;
-    A.delta_only = 1;
-    A.tw = ctx->tw.as<float2>();
-    A.win = ctx->win.as<float>();
-    A.synth = ctx->synth.as<float>();
-    const size_t smem = fft_smem_bytes (kEmbedWarps) + 3 * kFrame * sizeof (float) + 2 * size_t (kEmbedWarps) * kEdge * sizeof (float2);
-    if (set_smem (ctx, k_embed, smem)) return 1;
-    const unsigned grid = unsigned ((A.n_proc + kEmbedTile - 1) / kEmbedTile);
-    PROF (ctx);
-    k_embed<<<grid, kEmbedWarps * 32, smem, ctx->stream>>> (A);
-    LAUNCH_CHECK ("k_embed");
-  }
-  /* 3. out_resampler (src/wmadd.cc:401-406) */
-  J.in = ctx->rs_out.as<float>(); J.out = ctx->pcm_rs.as<float>(); J.n_in = n44; J.n_stop = LLONG_MAX / 4; J.n_out = (long long) n_emit;
-  J.step = step_out; J.h = h_out; J.coef = coef_out;
-  if (launch_resample (ctx, { J }, channels))
-    return 1;
-  /* 4. mix + limiter at the input rate (src/wmadd.cc:553-569) */
-  long long n_lim_blocks = 0;
-  if (limiter_block > 0)
-    {
-      n_lim_blocks = (long long) ((n_emit + limiter_block - 1) / limiter_block) + 1;
-      CK (ctx->peaks.reserve (n_lim_blocks * sizeof (unsigned)));
-      CK (cudaMemsetAsync (ctx->peaks.p, 0, n_lim_blocks * sizeof (unsigned), ctx->stream));
-    }
-  if (snr_power)
-    {
-      CK (ctx->snr.reserve (2 * sizeof (double)));
-      CK (cudaMemsetAsync (ctx->snr.p, 0, 2 * sizeof (double), ctx->stream));
-    }
-  PROF (ctx);
-  k_mix_peaks<<<unsigned ((n_emit + 255) / 256), 256, 0, ctx->stream>>> (d_in, (long long) n_frames, ctx->pcm_rs.as<float>(), (long long) n_emit, channels, d_out,
-                                                                         limiter_block, limiter_ceiling, ctx->peaks.as<unsigned>(), snr_power ? ctx->snr.as<double>() : nullptr);
-  LAUNCH_CHECK ("k_mix_peaks");
-  if (limiter_block > 0)
-    {
-      PROF (ctx);
-      k_limiter<<<unsigned ((n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter)), 256, 0, ctx->stream>>> (d_out, 0, (long long) n_frames, channels, limiter_block, limiter_ceiling,
-                                                                            ctx->peaks.as<unsigned>(), n_lim_blocks, 0);
-      LAUNCH_CHECK ("k_limiter");
-    }
-  if (!out_dev)
-    CK (cudaMemcpyAsync (out, d_out, n_val * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
-  if (snr_power)
-    CK (cudaMemcpyAsync (snr_power, ctx->snr.p, 2 * sizeof (double), cudaMemcpyDeviceToHost, ctx->stream));
-  if (!out_dev || snr_power)
-    CK (cudaStreamSynchronize (ctx->stream));
-  return 0;
-}
-
-/* ---------------------------------------------------------------- batched embed at any sample rate */
+/* ---------------------------------------------------------------- batched embed */
 
 namespace {
 
@@ -2837,18 +2629,21 @@ awm_batch_rates_validate (const awm_batch_item *items, size_t n_items, size_t n_
   return why[0] ? 1 : 0;
 }
 
+namespace {
+
+/* awm_embed_batch, awm_embed_batch_offsets and awm_embed_batch_rates after their own argument checks (name: the error prefix).
+ * sample_rates NULL: every item is at mark_sample_rate; zero_frames NULL: every item starts a stream.  Items at mark_sample_rate
+ * use limiter_block44, the others rate * limiter_ms / 1000. */
 int
-awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                       const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate, int frames_pad_start,
-                       double water_delta, int limiter_ms, float limiter_ceiling, double *snr_power, size_t scratch_bytes)
+embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+             const uint8_t *coded_bits, const uint64_t *zero_frames, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate,
+             int frames_pad_start, double water_delta, int limiter_block44, int limiter_ms, float limiter_ceiling, double *snr_power,
+             size_t scratch_bytes)
 {
-  char why[240];
-  if (awm_batch_rates_validate (items, n_items, n_values, sample_rates, n_emit, mark_sample_rate, why, sizeof (why)))
-    return fail (ctx, "awm_embed_batch_rates: %s", why);
   if (!ctx->roles_fpb)
-    return fail (ctx, "awm_embed_batch_rates: awm_set_embed_roles has not been called");
-  if ((n_items && (!coded_bits || !n_emit)) || (n_values && (!in_v || !out_v)) || limiter_ms < 0)
-    return fail (ctx, "awm_embed_batch_rates: bad arguments");
+    return fail (ctx, "%s: awm_set_embed_roles has not been called", name);
+  if ((n_items && (!coded_bits || (sample_rates && !n_emit))) || (n_values && (!in_v || !out_v)) || limiter_ms < 0)
+    return fail (ctx, "%s: bad arguments", name);
   if (snr_power)
     std::fill (snr_power, snr_power + 2 * n_items, 0.0);
   if (n_values == 0)
@@ -2859,13 +2654,14 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
   float *d_out;
   if (batch_images (ctx, in_v, out_v, s16, n_values, &d_in, &d_out))
     return 1;
+  auto resampled = [&] (size_t i) { return sample_rates && sample_rates[i] != mark_sample_rate; };
   auto block_of = [&] (int rate) { return int ((long long) rate * limiter_ms / 1000); };      // add_watermark_buffer's limiter block
 
   /* filter tables of every resampled rate, all fetched before any is used: coef_table empties its cache when it is full */
   struct Filters { const float *coef_in = nullptr, *coef_out = nullptr; int h_in = 0, h_out = 0; };
   std::map<int, Filters> filters;
   for (size_t i = 0; i < n_items; i++)
-    if (items[i].n_frames && sample_rates[i] != mark_sample_rate)
+    if (items[i].n_frames && resampled (i))
       filters[sample_rates[i]];
   if (coef_cache_room (ctx, 2 * filters.size()))
     return 1;
@@ -2874,7 +2670,7 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
         coef_table (ctx, double (f.first) / mark_sample_rate, 16, &f.second.coef_out, &f.second.h_out))
       return 1;
 
-  /* work lists.  Items at the watermark rate: one k_embed_batch pass as in awm_embed_batch.  The others: consecutive waves whose
+  /* work lists.  Items at the watermark rate: one k_embed_batch pass, with their stream offsets.  The others: consecutive waves whose
    * scratch (input and watermark signal at the watermark rate, 2 x n44 x C floats per item) stays within scratch_bytes; an item
    * larger than that runs alone.  A wave's scratch holds the inputs of all its items, then their watermark signals. */
   struct Wave { size_t b0 = 0, r0 = 0, r1 = 0, values = 0; long long n_tiles = 0, n_rs = 0, n_mix = 0, n_lim = 0; };
@@ -2882,15 +2678,14 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
   std::vector<RateItem> rlist;
   std::vector<size_t> soff;                 // offset of rlist[k] in its wave's input half of the scratch
   std::vector<Wave> waves;
-  const int block44 = block_of (mark_sample_rate);
   long long n_tiles44 = 0, n_lim44 = 0, n_peaks = 0, unused = 0;
   uint64_t covered = 0;
   for (size_t i = 0; i < n_items; i++)
     {
       covered += items[i].n_frames * uint64_t (items[i].channels);
-      if (items[i].n_frames && sample_rates[i] == mark_sample_rate)
-        blist.push_back (batch_entry ((long long) items[i].value_offset, (long long) items[i].n_frames, items[i].channels, int (i), block44,
-                                      n_tiles44, n_lim44, n_peaks));
+      if (items[i].n_frames && !resampled (i))
+        blist.push_back (batch_entry ((long long) items[i].value_offset, (long long) items[i].n_frames, items[i].channels, int (i), limiter_block44,
+                                      n_tiles44, n_lim44, n_peaks, zero_frames ? (long long) zero_frames[i] : 0));
     }
   const size_t n_list44 = blist.size();
   const size_t cap = scratch_bytes ? scratch_bytes : kBatchDefaultScratch;
@@ -2898,9 +2693,9 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
   for (size_t i = 0; i < n_items; i++)
     {
       const awm_batch_item& bi = items[i];
-      const int rate = sample_rates[i];
-      if (!bi.n_frames || rate == mark_sample_rate)
+      if (!bi.n_frames || !resampled (i))
         continue;
+      const int rate = sample_rates[i];
       const Filters& f = filters[rate];
       RateItem R = {};
       R.in = d_in + bi.value_offset;
@@ -2909,7 +2704,7 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
       R.n_emit = (long long) n_emit[i];
       R.C = bi.channels;
       R.item = int (i);
-      R.step_in = 1.0 / (double (mark_sample_rate) / rate);      // as awm_embed_resampled: 1 / r_in, 1 / r_out
+      R.step_in = 1.0 / (double (mark_sample_rate) / rate);      // 1 / r_in, 1 / r_out: the ratios of the add loop's two resamplers
       R.step_out = 1.0 / (double (rate) / mark_sample_rate);
       R.h_in = f.h_in;
       R.h_out = f.h_out;
@@ -2917,7 +2712,7 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
       R.coef_out = f.coef_out;
       R.n44 = resampled_n44 (n_emit[i], R.step_out, R.h_out);
       R.limiter_block = block_of (rate);
-      R.n_blocks = R.limiter_block > 0 ? (R.n_emit + R.limiter_block - 1) / R.limiter_block + 1 : 0;   // as awm_embed_resampled's
+      R.n_blocks = R.limiter_block > 0 ? (R.n_emit + R.limiter_block - 1) / R.limiter_block + 1 : 0;   // every block the mixer reaches
       R.peak0 = n_peaks;
       n_peaks += R.n_blocks;
       const size_t values = size_t (R.n44) * size_t (R.C);
@@ -2936,7 +2731,7 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
       w.n_mix += (R.n_emit + kRateCta - 1) / kRateCta;
       if (R.limiter_block > 0)
         w.n_lim += (R.n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter);
-      /* WatermarkGen::run on the scratch copy: awm_embed_resampled's k_embed with n_frames = n44, no limiter, no --snr */
+      /* WatermarkGen::run on every 1024-frame of the scratch copy (src/wmadd.cc:394-399): n_frames = n44, no limiter, no --snr */
       blist.push_back (batch_entry ((long long) w.values, R.n44, R.C, int (i), 0, w.n_tiles, unused, unused));
       soff.push_back (w.values);
       w.values += values;
@@ -2948,7 +2743,7 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
   for (const Wave& w : waves)
     too_large = too_large || std::max ({ w.n_tiles, w.n_rs, w.n_mix, w.n_lim }) >= INT_MAX;
   if (too_large)
-    return fail (ctx, "awm_embed_batch_rates: batch too large for one launch per step");
+    return fail (ctx, "%s: batch too large for one launch per step", name);
   if (covered < n_values)               /* values between items pass through unchanged */
     CK (cudaMemcpyAsync (d_out, d_in, n_values * sizeof (float), cudaMemcpyDeviceToDevice, ctx->stream));
   if (!blist.empty())
@@ -2982,8 +2777,8 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
         }
       double *d_snr = snr_power ? ctx->snr.as<double>() : nullptr;
       const BatchItem *d_b = ctx->batch_items.as<BatchItem>();
-      if (n_list44 && launch_embed_batch (ctx, d_in, d_out, d_b, int (n_list44), n_tiles44, n_lim44, frames_pad_start, water_delta, block44,
-                                          limiter_ceiling, d_snr, 0))
+      if (n_list44 && launch_embed_batch (ctx, d_in, d_out, d_b, int (n_list44), n_tiles44, n_lim44, frames_pad_start, water_delta, limiter_block44,
+                                          limiter_ceiling, d_snr, 0, zero_frames != nullptr))
         return 1;
       for (const Wave& w : waves)
         {
@@ -3007,6 +2802,47 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
         }
     }
   return batch_finish (ctx, out_v, s16, n_values, d_out, snr_power, blist.empty() ? 0 : n_items);
+}
+
+} // namespace
+
+int
+awm_embed_batch (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                 const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling,
+                 double *snr_power)
+{
+  char why[160];
+  if (awm_batch_validate (items, n_items, n_values, why, sizeof (why)))
+    return fail (ctx, "awm_embed_batch: %s", why);
+  return embed_batch ("awm_embed_batch", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, nullptr, nullptr, nullptr, 0,
+                      frames_pad_start, water_delta, limiter_block, 0, limiter_ceiling, snr_power, 0);
+}
+
+int
+awm_embed_batch_offsets (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                         const uint64_t *zero_frames, const uint8_t *coded_bits, int frames_pad_start, double water_delta, int limiter_block,
+                         float limiter_ceiling, double *snr_power)
+{
+  if (n_items && !zero_frames)
+    return fail (ctx, "awm_embed_batch_offsets: zero_frames list is NULL");
+  char why[160];
+  if (batch_offsets_check (items, n_items, n_values, zero_frames, false, why, sizeof (why)))
+    return fail (ctx, "awm_embed_batch_offsets: %s", why);
+  return embed_batch ("awm_embed_batch_offsets", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, zero_frames, nullptr, nullptr, 0,
+                      frames_pad_start, water_delta, limiter_block, 0, limiter_ceiling, snr_power, 0);
+}
+
+int
+awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                       const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate, int frames_pad_start,
+                       double water_delta, int limiter_ms, float limiter_ceiling, double *snr_power, size_t scratch_bytes)
+{
+  char why[240];
+  if (awm_batch_rates_validate (items, n_items, n_values, sample_rates, n_emit, mark_sample_rate, why, sizeof (why)))
+    return fail (ctx, "awm_embed_batch_rates: %s", why);
+  return embed_batch ("awm_embed_batch_rates", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, nullptr, sample_rates, n_emit,
+                      mark_sample_rate, frames_pad_start, water_delta, int ((long long) mark_sample_rate * limiter_ms / 1000), limiter_ms,
+                      limiter_ceiling, snr_power, scratch_bytes);
 }
 
 /* ---------------------------------------------------------------- speed scan */

@@ -175,47 +175,6 @@ k_gather (const float *__restrict__ src, const unsigned long long *__restrict__ 
     dst[k] = __ldg (src + idx[k]);
 }
 
-// out[i] = orig[i] + wm[i] for the frames the add loop emits (src/wmadd.cc:548-566 with a WatermarkResampler): orig is zero
-// beyond n_in; per limiter block the peak of |out| (only peaks above the ceiling matter, Limiter::block_max starts at the
-// ceiling) and the --snr sums.  Values are stored for i < n_in only, the limiter rescales them in place afterwards.
-__global__ void __launch_bounds__ (256)
-k_mix_peaks (const float *__restrict__ orig, long long n_in, const float *__restrict__ wm, long long n_emit, int C, float *__restrict__ out,
-             int limiter_block, float ceiling, unsigned *__restrict__ peaks, double *__restrict__ snr)
-{
-  const long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x;
-  double sd = 0, ss = 0;
-  if (i < n_emit)
-    {
-      float mx = 0.f;
-      for (int c = 0; c < C; c++)
-        {
-          const float o = i < n_in ? __ldg (orig + i * C + c) : 0.f;
-          const float w = __ldg (wm + i * C + c);
-          const float y = __fadd_rn (w, o);
-          if (i < n_in)
-            out[i * C + c] = y;
-          mx = fmaxf (mx, fabsf (y));
-          sd += double (w) * double (w);
-          ss += double (o) * double (o);
-        }
-      if (limiter_block > 0 && mx > ceiling)
-        atomicMax (peaks + i / limiter_block, __float_as_uint (mx));
-    }
-  if (snr)
-    {
-      for (int d = 16; d > 0; d >>= 1)
-        {
-          sd += __shfl_xor_sync (0xffffffffu, sd, d);
-          ss += __shfl_xor_sync (0xffffffffu, ss, d);
-        }
-      if ((threadIdx.x & 31) == 0 && (sd != 0 || ss != 0))
-        {
-          atomicAdd (snr, sd);
-          atomicAdd (snr + 1, ss);
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------- speed scan
 
 constexpr int kSpeedFrame = 512;           // Params::frame_size / 2          (src/wmspeed.cc:209)

@@ -58,6 +58,18 @@ resampled_add_plan (size_t n_frames, int sample_rate, bool limiter_on, size_t li
     }
 }
 
+/* the "Data Blocks" and --snr values of an add loop that made `runs` WatermarkGen::run calls with the given --snr sums */
+static AddStats
+add_stats (size_t runs, double snr_delta, double snr_signal)
+{
+  const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
+  const int blocks = int ((f0 + runs) / fpb - f0 / fpb);
+  AddStats s;
+  s.data_blocks = std::max (blocks - 1, 0);         // the first (partial B) block is padding
+  s.snr_db = snr_delta > 0 ? 10 * log10 (snr_signal / snr_delta) : INFINITY;
+  return s;
+}
+
 static void
 info_format (const string& label, const RawFormat& format)
 {
@@ -73,11 +85,6 @@ add_watermark_buffer (const Key& key, const float *in, float *out, size_t n_fram
   const vector<int> bitvec = parse_payload (bits);
   if (bitvec.empty())
     return 1;
-  awm_ctx *ctx = Engine::ctx();
-  if (!ctx || !Engine::set_embed_tables (key, bitvec))
-    return 1;
-  const int limiter_block = Params::test_no_limiter ? 0 : int (sample_rate * int (Params::limiter_block_size_ms) / 1000);
-  double snr_power[2] = { 0, 0 };
   if (sample_rate != Params::mark_sample_rate)
     {
       if (first_frame_number)
@@ -85,23 +92,21 @@ add_watermark_buffer (const Key& key, const float *in, float *out, size_t n_fram
           error ("audiowmark: sharded embedding is only available at %d Hz\n", Params::mark_sample_rate);
           return 1;
         }
-      size_t n_emit = 0, runs = 0;
-      resampled_add_plan (n_frames, sample_rate, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000, n_emit, runs);
-      if (awm_embed_resampled (ctx, in, out, n_frames, n_channels, sample_rate, Params::mark_sample_rate, std::max (n_emit, n_frames), Params::frames_pad_start,
-                               Params::water_delta, limiter_block, Params::limiter_ceiling, (Params::snr || stats) ? snr_power : nullptr))
-        {
-          error ("audiowmark: embedding failed: %s\n", awm_last_error (ctx));
-          return 1;
-        }
+      /* a batch of one item: the embed at other rates exists in batched form only */
+      const awm_batch_item item = { 0, n_frames, n_channels };
+      vector<AddStats> item_stats;
+      if (add_watermark_batch_rates (key, in, out, false, n_frames * size_t (n_channels), &item, 1, { bits }, &sample_rate, 0,
+                                     stats ? &item_stats : nullptr))
+        return 1;
       if (stats)
-        {
-          const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
-          const int blocks = int ((f0 + runs) / fpb - f0 / fpb);
-          stats->data_blocks = std::max (blocks - 1, 0);
-          stats->snr_db = snr_power[0] > 0 ? 10 * log10 (snr_power[1] / snr_power[0]) : INFINITY;
-        }
+        *stats = item_stats[0];
       return 0;
     }
+  awm_ctx *ctx = Engine::ctx();
+  if (!ctx || !Engine::set_embed_tables (key, bitvec))
+    return 1;
+  const int limiter_block = Params::test_no_limiter ? 0 : int (sample_rate * int (Params::limiter_block_size_ms) / 1000);
+  double snr_power[2] = { 0, 0 };
   if (awm_embed (ctx, in, out, n_frames, n_channels, first_frame_number, Params::frames_pad_start, Params::water_delta,
                  limiter_block, Params::limiter_ceiling, (Params::snr || stats) ? snr_power : nullptr))
     {
@@ -109,13 +114,7 @@ add_watermark_buffer (const Key& key, const float *in, float *out, size_t n_fram
       return 1;
     }
   if (stats)
-    {
-      const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
-      const size_t runs = gen_runs (n_frames, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000);
-      const int blocks = int ((f0 + runs) / fpb - f0 / fpb);
-      stats->data_blocks = std::max (blocks - 1, 0);         // the first (partial B) block is padding
-      stats->snr_db = snr_power[0] > 0 ? 10 * log10 (snr_power[1] / snr_power[0]) : INFINITY;
-    }
+    *stats = add_stats (gen_runs (n_frames, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000), snr_power[0], snr_power[1]);
   return 0;
 }
 
@@ -145,13 +144,7 @@ add_watermark_buffer_s16 (const Key& key, const int16_t *in, int16_t *out, size_
       return 1;
     }
   if (stats)
-    {
-      const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
-      const size_t runs = gen_runs (n_frames, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000);
-      const int blocks = int ((f0 + runs) / fpb - f0 / fpb);
-      stats->data_blocks = std::max (blocks - 1, 0);
-      stats->snr_db = snr_power[0] > 0 ? 10 * log10 (snr_power[1] / snr_power[0]) : INFINITY;
-    }
+    *stats = add_stats (gen_runs (n_frames, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000), snr_power[0], snr_power[1]);
   return 0;
 }
 
@@ -202,15 +195,12 @@ add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t
   if (stats)
     {
       stats->resize (n_items);
-      const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
       for (size_t i = 0; i < n_items; i++)
         {
           /* as add_watermark_windowed: the loop runs over the whole stream, silent prefix included */
           const size_t n_stream = items[i].n_frames + (zero_frames ? zero_frames[i] : 0);
-          const size_t runs = gen_runs (n_stream, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000);
-          const int blocks = int ((f0 + runs) / fpb - f0 / fpb);
-          (*stats)[i].data_blocks = std::max (blocks - 1, 0);
-          (*stats)[i].snr_db = snr_power[2 * i] > 0 ? 10 * log10 (snr_power[2 * i + 1] / snr_power[2 * i]) : INFINITY;
+          (*stats)[i] = add_stats (gen_runs (n_stream, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000),
+                                   snr_power[2 * i], snr_power[2 * i + 1]);
         }
     }
   return 0;
@@ -265,13 +255,8 @@ add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, 
   if (stats)
     {
       stats->resize (n_items);
-      const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
       for (size_t i = 0; i < n_items; i++)
-        {
-          const int blocks = int ((f0 + runs[i]) / fpb - f0 / fpb);
-          (*stats)[i].data_blocks = std::max (blocks - 1, 0);
-          (*stats)[i].snr_db = snr_power[2 * i] > 0 ? 10 * log10 (snr_power[2 * i + 1] / snr_power[2 * i]) : INFINITY;
-        }
+        (*stats)[i] = add_stats (runs[i], snr_power[2 * i], snr_power[2 * i + 1]);
     }
   return 0;
 }
@@ -389,13 +374,7 @@ add_watermark_windowed (const Key& key, const std::function<Error (vector<float>
   if (frames_written)
     *frames_written = written;
   if (stats)
-    {
-      const size_t fpb = frames_per_block(), f0 = 2 * fpb - Params::frames_pad_start;
-      const size_t runs = gen_runs (p1, !Params::test_no_limiter, L);
-      const int blocks = int ((f0 + runs) / fpb - f0 / fpb);
-      stats->data_blocks = std::max (blocks - 1, 0);         // the first (partial B) block is padding
-      stats->snr_db = snr_delta > 0 ? 10 * log10 (snr_signal / snr_delta) : INFINITY;
-    }
+    *stats = add_stats (gen_runs (p1, !Params::test_no_limiter, L), snr_delta, snr_signal);
   return 0;
 }
 
@@ -432,7 +411,7 @@ add_stream_watermark (const Key& key, AudioInputStream *in_stream, AudioOutputSt
   Error err;
   if (in_stream->sample_rate() != Params::mark_sample_rate)
     {
-      /* other sample rates go through the resamplers around the embedder (awm_embed_resampled): whole stream at once */
+      /* other sample rates go through the resamplers around the embedder (a one-item awm_embed_batch_rates): whole stream at once */
       if (zero_frames)
         {
           error ("audiowmark: stream offsets are only supported at %d Hz\n", Params::mark_sample_rate);

@@ -211,10 +211,14 @@ int awm_embed_batch_offsets (awm_ctx *ctx, const void *in, void *out, int is_s16
  * n_emit is not NULL, n_emit[i] >= n_frames of every resampled item; else nonzero with the reason in err.  Needs no device. */
 int awm_batch_rates_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const int *sample_rates, const uint64_t *n_emit,
                               int mark_sample_rate, char *err, size_t err_cap);
-/* awm_embed_batch for items that each have their own sample rate.  Item i comes out bit identical to what `add` of that item alone
- * computes: awm_embed for sample_rates[i] == mark_sample_rate, awm_embed_resampled (n_emit[i], limiter block
- * sample_rates[i] * limiter_ms / 1000) for any other rate; 16 bit items as the float path between k_s16_to_f32 and k_f32_to_s16.
- * n_emit: [n_items], the frames awm_embed_resampled takes (resampled_add_plan on the host); ignored at mark_sample_rate.
+/* awm_embed_batch for items that each have their own sample rate.  Item i comes out as `add` of that item alone: awm_embed for
+ * sample_rates[i] == mark_sample_rate; for any other rate the add loop (src/wmadd.cc:520-589) with a WatermarkResampler (:353-430):
+ * the input is resampled to mark_sample_rate, the watermark signal alone is generated there (WatermarkGen::run), resampled back and
+ * added to the untouched input (:548-566), and the limiter runs at the input rate (limiter block sample_rates[i] * limiter_ms / 1000).
+ * 16 bit items as the float path between k_s16_to_f32 and k_f32_to_s16.
+ * n_emit: [n_items], n_emit[i] >= n_frames = frames the reference loop pushes through the mixer before it stops (zero frames are fed
+ * after EOF until resamplers and limiter have delivered everything; resampled_add_plan on the host): they enter the --snr sums and
+ * the limiter's block peaks.  Ignored at mark_sample_rate.
  * limiter_ms = 0 disables the limiter.  snr_power (optional): [n_items][2].  Items at other rates run in consecutive waves whose
  * scratch (2 x n44 x channels floats per item, n44 = its length at mark_sample_rate) stays within scratch_bytes (0: 4 GiB); an item
  * larger than that runs alone.  The bound PCM (awm_pcm_bind) stays valid.  Everything else as awm_embed_batch. */
@@ -299,16 +303,6 @@ int awm_viterbi (awm_ctx *ctx, const float *raw_bits, size_t n_jobs, int n_msg_b
  * in/out: interleaved, host or device.  hlen = 16 everywhere in the reference.
  */
 int awm_resample (awm_ctx *ctx, const float *in, size_t n_in, int channels, double ratio, int hlen, float *out, size_t n_out);
-
-/* ---- embed for inputs that are not at the watermark rate: WatermarkResampler::run (src/wmadd.cc:353-430) inside the
- * add loop (:520-589).  The input is resampled to mark_sample_rate, the watermark signal alone is generated there
- * (WatermarkGen::run), resampled back and added to the untouched input; the limiter runs at the input rate
- * (limiter_block = sample_rate * ms / 1000).  n_emit >= n_frames = frames the reference loop pushes through the mixer
- * before it stops (zero frames are fed after EOF until resamplers and limiter have delivered everything): they enter the
- * --snr sums and the limiter's block peaks.  in/out: [n_frames][channels], host or device.
- */
-int awm_embed_resampled (awm_ctx *ctx, const float *in, float *out, size_t n_frames, int channels, int sample_rate, int mark_sample_rate,
-                         size_t n_emit, int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling, double *snr_power);
 
 /* resample_ratio (wav_data, speed, ...) of decode() (src/wmget.cc:916) without leaving the device: the bound PCM is
  * resampled by `ratio` into a context-owned buffer of n_out frames, which becomes the bound PCM; awm_pcm_pop restores

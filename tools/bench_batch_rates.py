@@ -3,7 +3,8 @@
 awm_embed_batch_rates, INTEGRATION §4b), against a loop of per-item hostapi.add(..., sample_rate=r) over the same items.
 
 workloads  1024 x 10 s mono at 48 kHz (short clips: per-call overhead), 128 x 3 min stereo at 48 kHz (long clips: bandwidth, several
-           scratch waves), 384 x 30 s stereo split evenly over 32 / 44.1 / 48 kHz (a mixed-rate library); uniform noise at -6 dBFS,
+           scratch waves), 384 x 30 s stereo split evenly over 32 / 44.1 / 48 kHz (a mixed-rate library), 1 x 60 min stereo at 48 kHz
+           (one long soundtrack: the single `add` is a one-item batch, so loop and batch run the same path); uniform noise at -6 dBFS,
            a random payload per item
 residency  PCM resident in HBM (one packed float32 tensor; the loop passes device pointers into it)
 timing     host wall time around each pass; both passes end in a synchronise; the two alternate within every step
@@ -27,7 +28,8 @@ from bench_batch import gpu_card  # noqa: E402
 
 WORKLOADS = [("1024x10s_mono_48k", 1024, 10.0, 1, (48000,)),
              ("128x3min_stereo_48k", 128, 180.0, 2, (48000,)),
-             ("384x30s_stereo_32k_44k_48k", 384, 30.0, 2, (32000, 44100, 48000))]
+             ("384x30s_stereo_32k_44k_48k", 384, 30.0, 2, (32000, 44100, 48000)),
+             ("1x60min_stereo_48k", 1, 3600.0, 2, (48000,))]
 
 
 def main():
