@@ -1717,13 +1717,22 @@ awm_sync_peaks (awm_ctx *ctx, double min_abs_quality, awm_search_score *out, siz
   return 0;
 }
 
-/* force: -1 = default kernel choice, 0 = sliding DFT, 1 = fresh FFT per offset.  With q_out the per-offset qualities of that
- * kernel are written ([n_scores][65], invalid offsets flagged 0 in valid_out) and the scores are left alone.  With rescored_out
- * ([n_scores][65]) the sliding pass runs and the offsets k_refine_rank picks for exact re-scoring are flagged 1. */
+/* what a refine call hands back */
+enum class RefineOut
+{
+  Refined,          // the best fine offset of every candidate (awm_sync_refine)
+  Exact,            // the exact quality of every fine offset (awm_sync_refine_offsets, exact = 1)
+  Sliding,          // the sliding quality of every fine offset, the exact one above two channels (awm_sync_refine_offsets, exact = 0)
+  Rescored,         // the fine offsets that are scored exactly (awm_sync_refine_rescored)
+};
+
+/* Up to two channels a sliding DFT ranks the 65 fine offsets of every candidate and only the offsets it picks are scored exactly;
+ * above two channels, and for the exact per-offset qualities, every valid offset is.  Refined is written to `refined`, Exact and
+ * Sliding to q_out / valid_out ([n_scores][65], invalid offsets 0), Rescored to rescored_out ([n_scores][65], 1 = scored exactly). */
 static int
-refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last,
-             double water_delta, awm_search_score *scores, size_t n_scores, int force, double *q_out, unsigned char *valid_out,
-             unsigned char *rescored_out = nullptr)
+refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta,
+             const awm_search_score *scores, size_t n_scores, RefineOut want, awm_search_score *refined, double *q_out,
+             unsigned char *valid_out, unsigned char *rescored_out)
 {
   if (key_slot < 0 || key_slot >= AWM_MAX_KEYS || mode < 0 || mode > 1 || (n_scores && !scores))
     return fail (ctx, "awm_sync_refine: bad arguments");
@@ -1740,6 +1749,7 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
   const double norm_div = water_delta < 0.080 ? water_delta : 0.080;
 
   const size_t nc = n_scores;
+  const size_t np_max = nc * kOffsets;
   const int n_bits = t.n_bits;
   CK (ctx->cand_start.reserve (nc * sizeof (long long)));
   CK (ctx->cand_noff.reserve (nc * sizeof (int)));
@@ -1761,13 +1771,11 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
     }
   CK (cudaMemcpyAsync (ctx->cand_start.p, h_start, nc * sizeof (long long), cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaMemcpyAsync (ctx->cand_noff.p, h_noff, nc * sizeof (int), cudaMemcpyHostToDevice, ctx->stream));
-  if (rescored_out)
-    force = 0;
-  /* default: sliding DFT over the 65 offsets (awm_refine_slide.cuh); AWM_REFINE=fft selects the kernel that transforms every
-   * frame of every offset afresh (also used for more than two channels) */
-  static const bool force_fft = [] { const char *e = getenv ("AWM_REFINE"); return e && !strcmp (e, "fft"); } ();
-  const bool used_slide = force < 0 ? (ctx->pcm_ch <= 2 && !force_fft) : (force == 0 && ctx->pcm_ch <= 2);
-  if (used_slide)
+  const bool slide = ctx->pcm_ch <= 2 && want != RefineOut::Exact;        // the sliding pass is written for one and two channels
+  /* a float2 per (candidate, offset, entry) from the sliding pass, 2 x kUD band values per (pair, entry) from the exact re-score of up
+   * to all 65 offsets (k_refine_exact_fft_n): no reallocation between the kernels */
+  CK (ctx->r_ent_ud.reserve (np_max * t.n_ent * 2 * kUD * sizeof (float)));
+  if (slide)
     {
       if (!ctx->tw1024.p)
         {
@@ -1780,10 +1788,7 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
           CK (ctx->tw1024.reserve (tw.size() * sizeof (float2)));
           CK (cudaMemcpy (ctx->tw1024.p, tw.data(), tw.size() * sizeof (float2), cudaMemcpyHostToDevice));
         }
-      const size_t n_pairs = size_t (nc) * kOffsets * t.n_ent;
-      /* also what the exact re-score of up to all 65 offsets stores there (k_refine_exact_fft_n): no reallocation between the kernels */
-      CK (ctx->r_ent_ud.reserve (std::max (n_pairs * sizeof (float2), n_pairs * 2 * kUD * sizeof (float))));
-      CK (ctx->r_ent_flag.reserve (n_pairs));
+      CK (ctx->r_ent_flag.reserve (np_max * t.n_ent));
       const size_t smem = fft_smem_bytes (kSlideWarps);
       const long long jobs = (long long) nc * t.n_ent;
       const unsigned grid = unsigned ((jobs + kSlideWarps - 1) / kSlideWarps);
@@ -1813,21 +1818,6 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
         ctx->r_ud.as<float>(), ctx->r_cnt.as<int>(), ctx->rvalid.as<unsigned char>());
       LAUNCH_CHECK ("k_refine_reduce");
     }
-  else
-    {
-      const size_t smem = fft_smem_bytes (kRefineWarps) + kRefineWarps * 96 * sizeof (float);
-      if (set_smem (ctx, k_refine, smem)) return 1;
-      const long long jobs = (long long) nc * kOffsets * n_bits;
-      PROF (ctx);
-      k_refine<<<unsigned ((jobs + kRefineWarps - 1) / kRefineWarps), kRefineWarps * 32, smem, ctx->stream>>> (
-        ctx->pcm, (long long) ctx->pcm_frames, ctx->pcm_ch, ctx->cand_start.as<long long>(), ctx->cand_noff.as<int>(), int (nc),
-        t.ent.as<awm_sync_entry>(), t.off.as<int>(), n_bits, total, (long long) wav_first, (long long) wav_last,
-        ctx->r_ud.as<float>(), ctx->r_cnt.as<int>(), ctx->rvalid.as<unsigned char>(), ctx->tw.as<float2>(), ctx->win.as<float>());
-      LAUNCH_CHECK ("k_refine");
-      /* compulsory traffic: the sync frames of every candidate (+ the +-256 samples of the offsets) are read once -- the 65 offsets
-       * x 6 bits re-read them from L2 */
-      prof_bytes (ctx, double (nc) * double (t.n_ent) * (double (kFrame) + 512.0) * ctx->pcm_ch * sizeof (float));
-    }
   // sync_decode epilogue (src/syncfinder.cc:94-114,144-152) from the per-bit float sums
   auto quality_of = [&] (const float *ud, const int *cnt, size_t base) -> double
     {
@@ -1851,28 +1841,71 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
         sync_quality /= bit_count;
       return sync_quality / norm_div / 2.9;
     };
-  if (used_slide && !q_out)
+  /* the pair list (start, candidate, offset) and its length, and the sums of up to np_max pairs: those of k_refine_reduce
+   * ([candidate][65]) or those of the exact re-score (in list order) */
+  int *e_n = ctx->pin.get<int> (1);
+  int *e_cand = ctx->pin.get<int> (np_max);
+  int *e_off = ctx->pin.get<int> (np_max);
+  float *e_ud = ctx->pin.get<float> (np_max * n_bits * 2);
+  int *e_cnt = ctx->pin.get<int> (np_max * n_bits);
+  unsigned char *e_valid = ctx->pin.get<unsigned char> (np_max);
+  if (!e_n || !e_cand || !e_off || !e_ud || !e_cnt || !e_valid)
+    return fail (ctx, "awm_sync_refine: out of page-locked memory");
+  auto fetch_list = [&] () -> int
+    {
+      CK (cudaMemcpyAsync (e_n, ctx->ex_n.p, sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_cand, ctx->ex_cand.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_off, ctx->ex_off.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      return 0;
+    };
+  auto fetch_sums = [&] () -> int
+    {
+      CK (cudaMemcpyAsync (e_ud, ctx->r_ud.p, np_max * n_bits * 2 * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_cnt, ctx->r_cnt.p, np_max * n_bits * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaMemcpyAsync (e_valid, ctx->rvalid.p, np_max, cudaMemcpyDeviceToHost, ctx->stream));
+      CK (cudaStreamSynchronize (ctx->stream));
+      return 0;
+    };
+  // Exact / Sliding: the quality of the sums at `p` goes to offset `at` ([candidate][65]); offsets not written stay invalid
+  auto put_quality = [&] (size_t p, size_t at)
+    {
+      valid_out[at] = e_valid[p];
+      q_out[at] = e_valid[p] ? quality_of (e_ud, e_cnt, p) : 0.0;
+    };
+  if (q_out)
+    {
+      std::fill (valid_out, valid_out + np_max, 0);
+      std::fill (q_out, q_out + np_max, 0.0);
+    }
+  if (slide && want == RefineOut::Sliding)
+    {
+      if (fetch_sums()) return 1;
+      for (size_t c = 0; c < nc; c++)
+        for (int o = 0; o < h_noff[c]; o++)
+          put_quality (c * kOffsets + o, c * kOffsets + o);
+      return 0;
+    }
+  CK (ctx->ex_start.reserve (np_max * sizeof (long long)));
+  CK (ctx->ex_cand.reserve (np_max * sizeof (int)));
+  CK (ctx->ex_off.reserve (np_max * sizeof (int)));
+  CK (ctx->ex_n.reserve (sizeof (int)));
+  if (slide)
     {
       /* The sliding DFT only RANKS the 65 offsets: every offset whose sliding score S lies within kVerifyMargin of the best sliding
-       * score is scored again with fresh FFTs in the reference's summation order (k_refine_exact_fft / _sum compute what k_refine
-       * computes), and the reference's rule picks among those exact values E.  If |S - E| <= d for all offsets, the exact arg-max o*
-       * satisfies S(o*) >= E(o*) - d >= E(o') - d >= S(o') - 2d for the sliding arg-max o', so with kVerifyMargin >= 2d the exact
-       * arg-max is always re-scored and index / quality are those of the exact kernel.  d is measured by
-       * tests/test_gpu_stages.py::test_sync_refine_vs_oracle (asserted < kVerifyMargin / 4 on all 65 offsets of every golden candidate); neighbouring offsets
-       * of a real peak differ by ~3e-3, so usually one or two offsets are re-scored.  The offset of the approx index itself is
-       * always re-scored: in the reference the search starts from the approx quality, which there IS the exact value of that
-       * offset (same transforms, same order of additions); ours comes from the entry-sum formulation and differs by ~1e-5
-       * relative, so the exact value takes its place below.  k_refine_rank picks the offsets on the device (the same rule as
-       * tests/test_gpu_refine_rank.py applies on the host), so the sliding sums never leave the GPU. */
+       * score is scored again with fresh FFTs in the reference's summation order (k_refine_exact_fft_n / _sum_n below), and the
+       * reference's rule picks among those exact values E.  If |S - E| <= d for all offsets, the exact arg-max o* satisfies
+       * S(o*) >= E(o*) - d >= E(o') - d >= S(o') - 2d for the sliding arg-max o', so with kVerifyMargin >= 2d the exact arg-max is
+       * always re-scored and index / quality are those of the exact re-score of every offset.  d is measured by
+       * tests/test_gpu_stages.py::test_sync_refine_vs_oracle (asserted < kVerifyMargin / 4 on all 65 offsets of every golden
+       * candidate); neighbouring offsets of a real peak differ by ~3e-3, so usually one or two offsets are re-scored.  The offset of the approx index itself is always re-scored: in the
+       * reference the search starts from the approx quality, which there IS the exact value of that offset (same transforms, same
+       * order of additions); ours comes from the entry-sum formulation and differs by ~1e-5 relative, so the exact value takes its
+       * place below.  k_refine_rank picks the offsets on the device (the same rule as tests/test_gpu_refine_rank.py applies on the
+       * host), so the sliding sums never leave the GPU. */
       constexpr double kVerifyMargin = 1e-3;
-      const size_t np_max = nc * kOffsets;
       CK (ctx->cand_score.reserve (nc * sizeof (awm_search_score)));
       CK (ctx->rank_keep.reserve (nc * 3 * sizeof (unsigned)));
       CK (ctx->rank_first.reserve (nc * sizeof (int)));
-      CK (ctx->ex_start.reserve (np_max * sizeof (long long)));
-      CK (ctx->ex_cand.reserve (np_max * sizeof (int)));
-      CK (ctx->ex_off.reserve (np_max * sizeof (int)));
-      CK (ctx->ex_n.reserve (sizeof (int)));
       awm_search_score *h_sc = ctx->pin.get<awm_search_score> (nc);
       if (!h_sc)
         return fail (ctx, "awm_sync_refine: out of page-locked memory");
@@ -1883,129 +1916,96 @@ refine_impl (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t 
         ctx->cand_score.as<awm_search_score>(), ctx->cand_start.as<long long>(), ctx->cand_noff.as<int>(), int (nc), n_bits, norm_div, kVerifyMargin,
         ctx->rank_keep.as<unsigned>(), ctx->rank_first.as<int>(), ctx->ex_start.as<long long>(), ctx->ex_cand.as<int>(), ctx->ex_off.as<int>(), ctx->ex_n.as<int>());
       LAUNCH_CHECK ("k_refine_rank");
-      int *e_n = ctx->pin.get<int> (1);
-      int *e_cand = ctx->pin.get<int> (np_max);
-      int *e_off = ctx->pin.get<int> (np_max);
-      if (!e_n || !e_cand || !e_off)
-        return fail (ctx, "awm_sync_refine: out of page-locked memory");
-      if (rescored_out)
-        {
-          CK (cudaMemcpyAsync (e_n, ctx->ex_n.p, sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-          CK (cudaMemcpyAsync (e_cand, ctx->ex_cand.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-          CK (cudaMemcpyAsync (e_off, ctx->ex_off.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-          CK (cudaStreamSynchronize (ctx->stream));
-          std::fill (rescored_out, rescored_out + nc * kOffsets, 0);
-          for (int p = 0; p < *e_n; p++)
-            rescored_out[size_t (e_cand[p]) * kOffsets + e_off[p]] = 1;
-          return 0;
-        }
-      if (!ctx->n_sms)
-        CK (cudaDeviceGetAttribute (&ctx->n_sms, cudaDevAttrMultiProcessorCount, ctx->device));
-      const size_t smem = fft_smem_bytes (kExactWarps) + kExactWarps * 96 * sizeof (float);
-      if (set_smem (ctx, k_refine_exact_fft_n, smem)) return 1;
-      const long long jobs_max = (long long) np_max * t.n_ent;
-      PROF (ctx);
-      k_refine_exact_fft_n<<<unsigned (std::min<long long> ((jobs_max + kExactWarps - 1) / kExactWarps, 4LL * ctx->n_sms)), kExactWarps * 32, smem, ctx->stream>>> (
-        ctx->pcm, (long long) ctx->pcm_frames, ctx->pcm_ch, ctx->ex_start.as<long long>(), ctx->ex_n.as<int>(), t.ent.as<awm_sync_entry>(), t.n_ent,
-        ctx->r_ent_ud.as<float>(), ctx->tw.as<float2>(), ctx->win.as<float>());
-      LAUNCH_CHECK ("k_refine_exact_fft_n");
-      /* the re-scored offsets of a candidate lie within 512 samples of each other: its sync frames are compulsory traffic once
-       * (and were read by the sliding pass a moment ago: they come from L2) */
-      prof_bytes (ctx, double (nc) * double (t.n_ent) * (double (kFrame) + 512.0) * ctx->pcm_ch * sizeof (float));
-      int max_bit_frames = 1;
-      for (int b = 0; b < n_bits; b++)
-        max_bit_frames = std::max (max_bit_frames, t.h_off[b + 1] - t.h_off[b]);
-      const size_t sum_smem = size_t (kExactSumWarps) * max_bit_frames * kUD * sizeof (float);
-      if (set_smem (ctx, k_refine_exact_sum_n, sum_smem)) return 1;
-      const long long sum_jobs_max = (long long) np_max * n_bits * 2;
-      PROF (ctx);
-      k_refine_exact_sum_n<<<unsigned (std::min<long long> ((sum_jobs_max + kExactSumWarps - 1) / kExactSumWarps, 16LL * ctx->n_sms)), kExactSumWarps * 32, sum_smem, ctx->stream>>> (
-        ctx->r_ent_ud.as<float>(), ctx->ex_start.as<long long>(), ctx->ex_n.as<int>(), (long long) ctx->pcm_frames, ctx->pcm_ch, t.ent.as<awm_sync_entry>(), t.n_ent,
-        t.off.as<int>(), n_bits, total, (long long) wav_first, (long long) wav_last, max_bit_frames, ctx->r_ud.as<float>(), ctx->r_cnt.as<int>(), ctx->rvalid.as<unsigned char>());
-      LAUNCH_CHECK ("k_refine_exact_sum_n");
-      /* one round trip: the list, its length and the exact sums (sized for the longest list the rank can write) */
-      float *e_ud = ctx->pin.get<float> (np_max * n_bits * 2);
-      int *e_cnt = ctx->pin.get<int> (np_max * n_bits);
-      unsigned char *e_valid = ctx->pin.get<unsigned char> (np_max);
-      if (!e_ud || !e_cnt || !e_valid)
-        return fail (ctx, "awm_sync_refine: out of page-locked memory");
-      CK (cudaMemcpyAsync (e_n, ctx->ex_n.p, sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-      CK (cudaMemcpyAsync (e_cand, ctx->ex_cand.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-      CK (cudaMemcpyAsync (e_off, ctx->ex_off.p, np_max * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-      CK (cudaMemcpyAsync (e_ud, ctx->r_ud.p, np_max * n_bits * 2 * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
-      CK (cudaMemcpyAsync (e_cnt, ctx->r_cnt.p, np_max * n_bits * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-      CK (cudaMemcpyAsync (e_valid, ctx->rvalid.p, np_max, cudaMemcpyDeviceToHost, ctx->stream));
-      CK (cudaStreamSynchronize (ctx->stream));
-      const size_t np = size_t (*e_n);
-      std::vector<double> best_quality (nc);
-      std::vector<uint64_t> best_index (nc);
-      for (size_t c = 0; c < nc; c++)
-        {
-          best_quality[c] = scores[c].raw_quality;
-          best_index[c] = scores[c].index;
-        }
-      for (size_t p = 0; p < np; p++)               // starting value: the exact quality at the approx index
-        if (e_valid[p] && uint64_t (h_start[e_cand[p]] + 8LL * e_off[p]) == scores[e_cand[p]].index)
-          best_quality[e_cand[p]] = quality_of (e_ud, e_cnt, p);
-      for (size_t p = 0; p < np; p++)               // per candidate in ascending offset order
-        if (e_valid[p])
-          {
-            const size_t c = size_t (e_cand[p]);
-            const double q = quality_of (e_ud, e_cnt, p);
-            if (fabs (q - scores[c].local_mean) > fabs (best_quality[c] - scores[c].local_mean))   // src/syncfinder.cc:436-440
-              {
-                best_quality[c] = q;
-                best_index[c] = uint64_t (h_start[c] + 8LL * e_off[p]);
-              }
-          }
-      for (size_t c = 0; c < nc; c++)
-        {
-          scores[c].index = best_index[c];
-          scores[c].raw_quality = best_quality[c];
-        }
-      return 0;
     }
-  const size_t n_ud = nc * kOffsets * n_bits * 2, n_cnt = nc * kOffsets * n_bits, n_val = nc * kOffsets;
-  float *h_ud = ctx->pin.get<float> (n_ud);
-  int *h_cnt = ctx->pin.get<int> (n_cnt);
-  unsigned char *h_valid = ctx->pin.get<unsigned char> (n_val);
-  if (!h_ud || !h_cnt || !h_valid)
-    return fail (ctx, "awm_sync_refine: out of page-locked memory");
-  CK (cudaMemcpyAsync (h_ud, ctx->r_ud.p, n_ud * sizeof (float), cudaMemcpyDeviceToHost, ctx->stream));
-  CK (cudaMemcpyAsync (h_cnt, ctx->r_cnt.p, n_cnt * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
-  CK (cudaMemcpyAsync (h_valid, ctx->rvalid.p, n_val, cudaMemcpyDeviceToHost, ctx->stream));
-  CK (cudaStreamSynchronize (ctx->stream));
-  if (q_out)
+  else
     {
+      /* every offset that gets a result (sync_fft returns nothing for a window past the end), in candidate order, offsets ascending;
+       * the exact kernels read the starts and the length */
+      long long *e_start = ctx->pin.get<long long> (np_max);
+      if (!e_start)
+        return fail (ctx, "awm_sync_refine: out of page-locked memory");
+      int n = 0;
       for (size_t c = 0; c < nc; c++)
-        for (int o = 0; o < kOffsets; o++)
-          {
-            const bool v = o < h_noff[c] && h_valid[c * kOffsets + o];
-            valid_out[c * kOffsets + o] = v ? 1 : 0;
-            q_out[c * kOffsets + o] = v ? quality_of (h_ud, h_cnt, c * kOffsets + o) : 0.0;
-          }
+        for (int o = 0; o < h_noff[c]; o++)
+          if (h_start[c] + 8LL * o + (long long) total * kFrame <= (long long) ctx->pcm_frames)
+            {
+              e_start[n] = h_start[c] + 8LL * o;
+              e_cand[n] = int (c);
+              e_off[n] = o;
+              n++;
+            }
+      *e_n = n;
+      CK (cudaMemcpyAsync (ctx->ex_start.p, e_start, n * sizeof (long long), cudaMemcpyHostToDevice, ctx->stream));
+      CK (cudaMemcpyAsync (ctx->ex_n.p, e_n, sizeof (int), cudaMemcpyHostToDevice, ctx->stream));
+    }
+  if (want == RefineOut::Rescored)
+    {
+      if (slide && fetch_list()) return 1;
+      CK (cudaStreamSynchronize (ctx->stream));
+      std::fill (rescored_out, rescored_out + np_max, 0);
+      for (int p = 0; p < *e_n; p++)
+        rescored_out[size_t (e_cand[p]) * kOffsets + e_off[p]] = 1;
       return 0;
     }
+  if (!ctx->n_sms)
+    CK (cudaDeviceGetAttribute (&ctx->n_sms, cudaDevAttrMultiProcessorCount, ctx->device));
+  const size_t smem = fft_smem_bytes (kExactWarps) + kExactWarps * 96 * sizeof (float);
+  if (set_smem (ctx, k_refine_exact_fft_n, smem)) return 1;
+  const long long jobs_max = (long long) np_max * t.n_ent;
+  PROF (ctx);
+  k_refine_exact_fft_n<<<unsigned (std::min<long long> ((jobs_max + kExactWarps - 1) / kExactWarps, 4LL * ctx->n_sms)), kExactWarps * 32, smem, ctx->stream>>> (
+    ctx->pcm, (long long) ctx->pcm_frames, ctx->pcm_ch, ctx->ex_start.as<long long>(), ctx->ex_n.as<int>(), t.ent.as<awm_sync_entry>(), t.n_ent,
+    ctx->r_ent_ud.as<float>(), ctx->tw.as<float2>(), ctx->win.as<float>());
+  LAUNCH_CHECK ("k_refine_exact_fft_n");
+  /* the re-scored offsets of a candidate lie within 512 samples of each other: its sync frames are compulsory traffic once
+   * (and were read by the sliding pass a moment ago: they come from L2) */
+  prof_bytes (ctx, double (nc) * double (t.n_ent) * (double (kFrame) + 512.0) * ctx->pcm_ch * sizeof (float));
+  int max_bit_frames = 1;
+  for (int b = 0; b < n_bits; b++)
+    max_bit_frames = std::max (max_bit_frames, t.h_off[b + 1] - t.h_off[b]);
+  const size_t sum_smem = size_t (kExactSumWarps) * max_bit_frames * kUD * sizeof (float);
+  if (set_smem (ctx, k_refine_exact_sum_n, sum_smem)) return 1;
+  const long long sum_jobs_max = (long long) np_max * n_bits * 2;
+  PROF (ctx);
+  k_refine_exact_sum_n<<<unsigned (std::min<long long> ((sum_jobs_max + kExactSumWarps - 1) / kExactSumWarps, 16LL * ctx->n_sms)), kExactSumWarps * 32, sum_smem, ctx->stream>>> (
+    ctx->r_ent_ud.as<float>(), ctx->ex_start.as<long long>(), ctx->ex_n.as<int>(), (long long) ctx->pcm_frames, ctx->pcm_ch, t.ent.as<awm_sync_entry>(), t.n_ent,
+    t.off.as<int>(), n_bits, total, (long long) wav_first, (long long) wav_last, max_bit_frames, ctx->r_ud.as<float>(), ctx->r_cnt.as<int>(), ctx->rvalid.as<unsigned char>());
+  LAUNCH_CHECK ("k_refine_exact_sum_n");
+  if (slide && fetch_list()) return 1;          // one round trip: the list the device wrote and the exact sums
+  if (fetch_sums()) return 1;
+  const size_t np = size_t (*e_n);
+  if (want != RefineOut::Refined)
+    {
+      for (size_t p = 0; p < np; p++)
+        put_quality (p, size_t (e_cand[p]) * kOffsets + e_off[p]);
+      return 0;
+    }
+  std::vector<double> best_quality (nc);
+  std::vector<uint64_t> best_index (nc);
   for (size_t c = 0; c < nc; c++)
     {
-      awm_search_score& sc = scores[c];
-      double best_quality = sc.raw_quality;
-      uint64_t best_index = sc.index;
-      const int o_self = int (((long long) sc.index - h_start[c]) / 8);      // starting value: the exact quality at the approx index (see above)
-      if (o_self < h_noff[c] && h_valid[c * kOffsets + o_self])
-        best_quality = quality_of (h_ud, h_cnt, c * kOffsets + o_self);
-      for (int o = 0; o < h_noff[c]; o++)
-        if (h_valid[c * kOffsets + o])
+      best_quality[c] = scores[c].raw_quality;
+      best_index[c] = scores[c].index;
+    }
+  for (size_t p = 0; p < np; p++)               // starting value: the exact quality at the approx index
+    if (e_valid[p] && uint64_t (h_start[e_cand[p]] + 8LL * e_off[p]) == scores[e_cand[p]].index)
+      best_quality[e_cand[p]] = quality_of (e_ud, e_cnt, p);
+  for (size_t p = 0; p < np; p++)               // per candidate in ascending offset order
+    if (e_valid[p])
+      {
+        const size_t c = size_t (e_cand[p]);
+        const double q = quality_of (e_ud, e_cnt, p);
+        if (fabs (q - scores[c].local_mean) > fabs (best_quality[c] - scores[c].local_mean))   // src/syncfinder.cc:436-440
           {
-            const double q = quality_of (h_ud, h_cnt, c * kOffsets + o);
-            if (fabs (q - sc.local_mean) > fabs (best_quality - sc.local_mean))   // src/syncfinder.cc:436-440
-              {
-                best_quality = q;
-                best_index = uint64_t (h_start[c] + 8LL * o);
-              }
+            best_quality[c] = q;
+            best_index[c] = uint64_t (h_start[c] + 8LL * e_off[p]);
           }
-      sc.index = best_index;
-      sc.raw_quality = best_quality;
+      }
+  for (size_t c = 0; c < nc; c++)
+    {
+      refined[c] = scores[c];
+      refined[c].index = best_index[c];
+      refined[c].raw_quality = best_quality[c];
     }
   return 0;
 }
@@ -2014,7 +2014,7 @@ int
 awm_sync_refine (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last,
                  double water_delta, awm_search_score *scores, size_t n_scores)
 {
-  return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, scores, n_scores, -1, nullptr, nullptr);
+  return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, scores, n_scores, RefineOut::Refined, scores, nullptr, nullptr, nullptr);
 }
 
 int
@@ -2023,8 +2023,8 @@ awm_sync_refine_rescored (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_fir
 {
   if (!rescored_out)
     return fail (ctx, "awm_sync_refine_rescored: bad arguments");
-  return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, const_cast<awm_search_score *> (scores), n_scores, 0,
-                      nullptr, nullptr, rescored_out);
+  return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, scores, n_scores, RefineOut::Rescored, nullptr, nullptr, nullptr,
+                      rescored_out);
 }
 
 int
@@ -2033,8 +2033,8 @@ awm_sync_refine_offsets (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_firs
 {
   if (!quality_out || !valid_out)
     return fail (ctx, "awm_sync_refine_offsets: bad arguments");
-  return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, const_cast<awm_search_score *> (scores), n_scores, exact ? 1 : 0,
-                      quality_out, valid_out);
+  return refine_impl (ctx, key_slot, mode, wav_first, wav_last, water_delta, scores, n_scores, exact ? RefineOut::Exact : RefineOut::Sliding,
+                      nullptr, quality_out, valid_out, nullptr);
 }
 
 /* ---------------------------------------------------------------- multi-GPU exchange

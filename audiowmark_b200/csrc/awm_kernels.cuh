@@ -482,72 +482,9 @@ k_peaks (const awm_search_score *__restrict__ scores, long long n, double floor_
     }
 }
 
-// =============================================================================================
-// SyncFinder::search_refine (src/syncfinder.cc:393-458): for candidate c and fine offset o
-// (sample cand_start[c] + 8*o) sync_fft of the wanted sync frames + sync_decode (start frame 0).
-// One warp = one (candidate, offset, sync bit): it walks the bit's sync frames in ascending frame order,
-// one FFT each, and accumulates umag / dmag in the reference's order (lane 0: up bands, lane 1: down
-// bands, sequential float adds), so no spectra are ever written to memory.
-// out_ud[((c*65 + o)*n_bits + bit)*2 + {0,1}] = umag, dmag; out_cnt = frames used; out_valid[c*65 + o].
-// =============================================================================================
+// SyncFinder::search_refine (src/syncfinder.cc:393-458) scores the fine offsets cand_start + 8*o, o < 65, of every candidate
+// (awm_refine_slide.cuh)
 constexpr int kOffsets = 65;
-constexpr int kRefineWarps = 10;      // 2 CTAs/SM = 20 warps: shared memory (transpose buffers) and 102 registers/thread both fit
-
-__global__ void __launch_bounds__ (kRefineWarps * 32, 2)
-k_refine (const float *__restrict__ pcm, long long n_frames, int C,
-          const long long *__restrict__ cand_start, const int *__restrict__ cand_noff, int n_cand,
-          const awm_sync_entry *__restrict__ g_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,
-          long long wav_first, long long wav_last,
-          float *__restrict__ out_ud, int *__restrict__ out_cnt, unsigned char *__restrict__ out_valid,
-          const float2 *g_tw, const float *g_win)
-{
-  extern __shared__ __align__ (16) unsigned char smem[];
-  FftSmem s = fft_smem_setup (smem, g_tw, g_win, kRefineWarps);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float *sband = s.extra + w * 96;                      // [81] per warp
-  const long long job = (long long) blockIdx.x * kRefineWarps + w;
-  if (job >= (long long) n_cand * kOffsets * n_bits)
-    return;
-  const int c = int (job / (kOffsets * n_bits));
-  const int o = int ((job / n_bits) % kOffsets);
-  const int bit = int (job % n_bits);
-  const long long fine = cand_start[c] + 8LL * o;
-  // sync_fft: an offset whose window would read past the end yields no result at all
-  const bool valid = o < cand_noff[c] && fine + (long long) total_frame_count * kFrame <= n_frames;
-  if (bit == 0 && lane == 0)
-    out_valid[c * kOffsets + o] = valid ? 1 : 0;
-  if (!valid)
-    return;
-  float mag = 0.f;                                      // lane 0: umag, lane 1: dmag
-  int cnt = 0;
-  const int e1 = g_bit_off[bit + 1];
-  for (int e = g_bit_off[bit]; e < e1; e++)
-    {
-      const awm_sync_entry *en = g_ent + e;
-      const long long start = fine + (long long) en->frame * kFrame;
-      const long long f_first = start * C, f_last = (start + kFrame) * C;
-      if (f_last < wav_first || f_first > wav_last)     // frame in digital silence: not counted
-        continue;
-      float acc[4];
-      frame_db_sum (pcm, n_frames, C, start, s, lane, acc);
-      bands_to_array (acc, lane, sband, 1);
-      __syncwarp();
-      if (lane < 2)
-        {
-          const uint8_t *idx = lane == 0 ? en->up : en->down;
-#pragma unroll 6
-          for (int i = 0; i < kUD; i++)
-            mag += sband[idx[i]];
-        }
-      cnt++;
-      __syncwarp();
-    }
-  const size_t ob = ((size_t) c * kOffsets + o) * n_bits + bit;
-  if (lane < 2)
-    out_ud[ob * 2 + lane] = mag;
-  if (lane == 0)
-    out_cnt[ob] = cnt;
-}
 
 // =============================================================================================
 // block decode, stage 1: FFTAnalyzer::fft_range (src/wmcommon.cc:123-141) reduced to what

@@ -44,7 +44,7 @@ k_refine_slide (const float *__restrict__ pcm, long long n_frames,
   const int c = int (job / n_ent), e = int (job % n_ent);
   const awm_sync_entry *en = g_ent + e;
   const long long p0 = cand_start[c] + (long long) en->frame * kFrame;      // first sample of this sync frame at offset 0
-  // offsets whose block would read past the end yield no result (sync_fft returns nothing): same rule as k_refine
+  // offsets whose block would read past the end yield no result (sync_fft returns nothing): same rule as k_refine_reduce
   long long n_valid = cand_noff[c];
   {
     const long long room = n_frames - (long long) total_frame_count * kFrame - cand_start[c];
@@ -330,7 +330,7 @@ k_refine_slide (const float *__restrict__ pcm, long long n_frames,
 }
 
 // per (candidate, offset, sync bit): add the per-frame sums in frame order, count the frames that were used
-// -> the layout k_refine writes (out_ud / out_cnt / out_valid), so the host side is unchanged
+// -> out_ud[((c*65 + o)*n_bits + bit)*2 + {0,1}] = umag, dmag; out_cnt = frames used; out_valid[c*65 + o]
 __global__ void
 k_refine_reduce (const float2 *__restrict__ ent_ud, const unsigned char *__restrict__ ent_flag, int n_cand, int n_ent,
                  const int *__restrict__ g_bit_off, int n_bits, const long long *__restrict__ cand_start, const int *__restrict__ cand_noff,
@@ -369,14 +369,14 @@ k_refine_reduce (const float2 *__restrict__ ent_ud, const unsigned char *__restr
 
 namespace awm {
 
-// ---- exact re-scoring of a few (candidate, offset) pairs picked by the sliding pass -------------------------------------------
-// k_refine computes the same thing with one warp per (pair, sync bit) walking 85 frames one after the other; for a handful of
-// pairs that is a long serial chain on a nearly empty GPU.  Here the transforms run in parallel (warp = one pair x one sync frame,
-// time-domain window and arithmetic of frame_db_sum, i.e. of the reference's sync_fft) and only the additions stay serial:
-// k_refine_exact_sum adds the stored band values of a bit in the reference's order (frames ascending, 30 up / 30 down bands each).
+// ---- exact scoring of a list of (candidate, offset) pairs: the ones the sliding pass picks, or every valid offset --------------
+// The transforms run in parallel (warp = one pair x one sync frame, time-domain window and arithmetic of frame_db_sum, i.e. of the
+// reference's sync_fft) and only the additions stay serial: k_refine_exact_sum_n adds the stored band values of a bit in the
+// reference's order (frames ascending, 30 up / 30 down bands each).  The list's length is written by the device (k_refine_rank) or
+// the host; a fixed grid walks the jobs.
 constexpr int kExactWarps = 8;
 
-/* one (pair, sync frame) job of k_refine_exact_fft */
+/* one (pair, sync frame) job of k_refine_exact_fft_n */
 __device__ __forceinline__ void
 refine_exact_fft_job (const float *__restrict__ pcm, long long n_frames, int C, const long long *__restrict__ pair_start,
                       const awm_sync_entry *__restrict__ g_ent, int n_ent, float *__restrict__ vals, const FftSmem& s, float *sband,
@@ -398,22 +398,6 @@ refine_exact_fft_job (const float *__restrict__ pcm, long long n_frames, int C, 
 }
 
 __global__ void __launch_bounds__ (kExactWarps * 32, 2)
-k_refine_exact_fft (const float *__restrict__ pcm, long long n_frames, int C, const long long *__restrict__ pair_start, int n_pairs,
-                    const awm_sync_entry *__restrict__ g_ent, int n_ent, float *__restrict__ vals /* [pair][entry][60] */,
-                    const float2 *g_tw, const float *g_win)
-{
-  extern __shared__ __align__ (16) unsigned char smem[];
-  FftSmem s = fft_smem_setup (smem, g_tw, g_win, kExactWarps);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float *sband = s.extra + w * 96;
-  const long long job = (long long) blockIdx.x * kExactWarps + w;
-  if (job >= (long long) n_pairs * n_ent)
-    return;
-  refine_exact_fft_job (pcm, n_frames, C, pair_start, g_ent, n_ent, vals, s, sband, lane, job);
-}
-
-/* the same for a pair list whose length the device wrote (k_refine_rank): a fixed grid walks the jobs */
-__global__ void __launch_bounds__ (kExactWarps * 32, 2)
 k_refine_exact_fft_n (const float *__restrict__ pcm, long long n_frames, int C, const long long *__restrict__ pair_start, const int *__restrict__ n_pairs,
                       const awm_sync_entry *__restrict__ g_ent, int n_ent, float *__restrict__ vals, const float2 *g_tw, const float *g_win)
 {
@@ -434,7 +418,7 @@ k_refine_exact_fft_n (const float *__restrict__ pcm, long long n_frames, int C, 
 // additions is what this kernel's time consists of, the loads no longer sit between them.
 constexpr int kExactSumWarps = 4;
 
-/* one (pair, sync bit, up / down) job of k_refine_exact_sum */
+/* one (pair, sync bit, up / down) job of k_refine_exact_sum_n */
 __device__ __forceinline__ void
 refine_exact_sum_job (const float *__restrict__ vals, const long long *__restrict__ pair_start, long long n_frames, int C,
                       const awm_sync_entry *__restrict__ g_ent, int n_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,
@@ -473,23 +457,6 @@ refine_exact_sum_job (const float *__restrict__ vals, const long long *__restric
     out_cnt[(size_t) p * n_bits + bit] = cnt;
 }
 
-__global__ void __launch_bounds__ (kExactSumWarps * 32)
-k_refine_exact_sum (const float *__restrict__ vals, const long long *__restrict__ pair_start, int n_pairs, long long n_frames, int C,
-                    const awm_sync_entry *__restrict__ g_ent, int n_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,
-                    long long wav_first, long long wav_last, int max_bit_frames,
-                    float *__restrict__ out_ud /* [pair][n_bits][2] */, int *__restrict__ out_cnt, unsigned char *__restrict__ out_valid)
-{
-  extern __shared__ __align__ (16) unsigned char smem[];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float *stage = reinterpret_cast<float *> (smem) + size_t (w) * max_bit_frames * kUD;
-  const int i = blockIdx.x * kExactSumWarps + w;
-  if (i >= n_pairs * n_bits * 2)
-    return;
-  refine_exact_sum_job (vals, pair_start, n_frames, C, g_ent, n_ent, g_bit_off, n_bits, total_frame_count, wav_first, wav_last,
-                        out_ud, out_cnt, out_valid, stage, lane, i);
-}
-
-/* the same for a pair list whose length the device wrote (k_refine_rank): a fixed grid walks the jobs */
 __global__ void __launch_bounds__ (kExactSumWarps * 32)
 k_refine_exact_sum_n (const float *__restrict__ vals, const long long *__restrict__ pair_start, const int *__restrict__ n_pairs, long long n_frames, int C,
                       const awm_sync_entry *__restrict__ g_ent, int n_ent, const int *__restrict__ g_bit_off, int n_bits, int total_frame_count,

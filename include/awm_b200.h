@@ -267,13 +267,15 @@ int awm_sync_refine (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, u
  * (src/syncfinder.cc:428-434), as the sliding-DFT kernel ranks them (exact = 0) or from fresh transforms in the reference's
  * summation order (exact = 1).  quality_out / valid_out: [n_scores][65]; offsets the reference gets no result for
  * (sync_fft returns nothing past the end of the signal) have valid 0.  awm_sync_refine re-scores every offset whose sliding
- * quality is within 1e-3 of the best exactly, so its result is that of the exact kernel as long as the two differ by < 5e-4. */
+ * quality is within 1e-3 of the best exactly, so its result is that of the exact kernel as long as the two differ by < 5e-4.
+ * On more than two channels there is no sliding pass: exact = 0 returns the exact qualities as well. */
 int awm_sync_refine_offsets (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta,
                              const awm_search_score *scores, size_t n_scores, int exact, double *quality_out, unsigned char *valid_out);
 
 /* measurement aid for the parity tests: the fine offsets awm_sync_refine re-scores exactly, as its ranking kernel picks them on the
  * device from the sliding qualities (every valid offset whose -|q - local_mean| is within 1e-3 of the smallest, plus the offset of the
- * approx index if it is valid).  rescored_out: [n_scores][65], 1 = re-scored. */
+ * approx index if it is valid).  On more than two channels every valid offset is scored exactly and flagged.
+ * rescored_out: [n_scores][65], 1 = re-scored; scores is only read. */
 int awm_sync_refine_rescored (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta,
                               const awm_search_score *scores, size_t n_scores, unsigned char *rescored_out);
 

@@ -833,7 +833,8 @@ class SyncFinder:
         return self.std_sort_desc(scores)[:n]
 
     # -- search_refine (syncfinder.cc:393-458)
-    def search_refine(self, samples, mode, scores, sb: SyncBits, key: Key):
+    def refine_qualities(self, samples, mode, index, sb: SyncBits, key: Key):
+        """the fine offsets search_refine scores around one approx index -> [(fine, quality or None if past the end)]"""
         P = self.P
         total = frames_per_block(P)
         first_block_end = total
@@ -846,16 +847,19 @@ class SyncFinder:
             if mode == CLIP:
                 want[first_block_end + bpg.sync_frame(f)] = 1
         out = []
+        start = max(int(index) - P.sync_search_step, 0)
+        for fine in range(start, int(index) + P.sync_search_step + 1, P.sync_search_fine):
+            db, have = self.sync_fft(samples, fine, total, want)
+            out.append((fine, None if db is None else float(self.sync_decode(sb, [0], db, have)[0])))
+        return out
+
+    def search_refine(self, samples, mode, scores, sb: SyncBits, key: Key):
+        out = []
         for sc in scores:
             best_q, best_i = sc.raw_quality, sc.index
-            start = max(int(sc.index) - P.sync_search_step, 0)
-            end = sc.index + P.sync_search_step
-            for fine in range(start, end + 1, P.sync_search_fine):
-                db, have = self.sync_fft(samples, fine, total, want)
-                if db is not None:
-                    q = float(self.sync_decode(sb, [0], db, have)[0])
-                    if abs(q - sc.local_mean) > abs(best_q - sc.local_mean):
-                        best_q, best_i = q, fine
+            for fine, q in self.refine_qualities(samples, mode, sc.index, sb, key):
+                if q is not None and abs(q - sc.local_mean) > abs(best_q - sc.local_mean):
+                    best_q, best_i = q, fine
             out.append(SearchScore(best_i, best_q, sc.local_mean))
         out.sort(key=lambda s: s.index)
         return out

@@ -206,16 +206,16 @@ def test_cli_reference_shell_tests(tmp_path):
 
 
 def test_cli_reference_order_kernels_give_the_same_answer(tmp_path):
-    """AWM_APPROX=ring / AWM_REFINE=fft select the kernels that keep the reference's exact float summation order (one thread per
-    start frame, one fresh FFT per fine offset); the default kernels (entry sums + gather, sliding DFT) must print the same
-    patterns, positions and three-digit qualities"""
+    """AWM_APPROX=ring selects the approx search kernel that keeps the reference's exact float summation order (one thread per
+    start frame); the default one (entry sums + gather) must print the same patterns, positions and three-digit qualities.
+    The refine always ends in the reference's order: test_gpu_stages.py::test_sync_refine_vs_oracle holds it to the oracle."""
     import subprocess
     cli = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "audiowmark_b200", "bin", "audiowmark")
     a, b = str(tmp_path / "in.wav"), str(tmp_path / "out.wav")
     subprocess.check_call([cli, "test-gen-noise", a, "200", "44100"])
     subprocess.check_call([cli, "add", "-q", a, b, "f0f0f0f0f0f0f0f0f0f0f0f0f0f0f0f0"])
     fast = subprocess.run([cli, "get", b], capture_output=True, text=True, check=True).stdout
-    env = dict(os.environ, AWM_APPROX="ring", AWM_REFINE="fft")
+    env = dict(os.environ, AWM_APPROX="ring")
     exact = subprocess.run([cli, "get", b], capture_output=True, text=True, check=True, env=env).stdout
     real = lambda out: [l for l in out.split("\n") if "f0f0f0f0f0f0f0f0f0f0f0f0f0f0f0f0" in l]
     assert len(real(fast)) == 5 and real(fast) == real(exact)

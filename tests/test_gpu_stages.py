@@ -152,7 +152,15 @@ def test_tensor_core_entry_sums_match_fp32_pipes(ctx, marked, monkeypatch):
 
 
 def test_sync_refine_vs_oracle(ctx, marked):
-    _, y = marked
+    """stereo, mono and three channels (stereo plus their mean): stereo and mono take the sliding pass, three channels score every
+    offset exactly"""
+    _, y2 = marked
+    for y in (y2, y2[:, :1], np.stack([y2[:, 0], y2[:, 1], 0.5 * (y2[:, 0] + y2[:, 1])], axis=1)):
+        refine_vs_oracle(ctx, np.ascontiguousarray(y, np.float32))
+
+
+def refine_vs_oracle(ctx, y):
+    channels = y.shape[1]
     ctx.pcm_bind(y)
     sf = O.SyncFinder(P)
     sf.first, sf.last = 0, y.size
@@ -167,17 +175,17 @@ def test_sync_refine_vs_oracle(ctx, marked):
     inp["raw_quality"] = [s.raw_quality for s in sel]
     inp["local_mean"] = [s.local_mean for s in sel]
     got = np.sort(ctx.sync_refine(inp, 0, capi.MODE_BLOCK), order="index")
-    assert len(got) == len(want)
+    assert len(got) == len(want), channels
     for g, w in zip(got, want):
-        assert int(g["index"]) == w.index, (g, w)               # sync positions are exact, not "within one fine step"
-        assert abs(g["raw_quality"] - w.raw_quality) < 2e-4
+        assert int(g["index"]) == w.index, (channels, g, w)     # sync positions are exact, not "within one fine step"
+        assert abs(g["raw_quality"] - w.raw_quality) < 2e-4, (channels, g, w)
         assert g["local_mean"] == w.local_mean
     # error bound behind the exactness claim (awm_capi.cu: kVerifyMargin = 1e-3): the sliding-DFT ranking S and the exact scores E
     # of all 65 offsets differ by less than half the margin, so the exact arg-max is always among the re-scored offsets
     S, vs = ctx.sync_refine_offsets(inp, exact=False)
     E, ve = ctx.sync_refine_offsets(inp, exact=True)
-    assert np.array_equal(vs, ve) and vs.sum() > 60 * (len(sel) - 2)
-    assert np.abs(S - E)[vs].max() < 5e-4 * 0.5, np.abs(S - E)[vs].max()
+    assert np.array_equal(vs, ve) and vs.sum() > 60 * (len(sel) - 2), channels
+    assert np.abs(S - E)[vs].max() < 5e-4 * 0.5, (channels, np.abs(S - E)[vs].max())
     # the result is the exact kernel's: the reference rule (start from the approx index, replace on strictly larger |q - mean|,
     # offsets ascending) applied to E alone gives the indices awm_sync_refine returns
     unsorted = ctx.sync_refine(inp, 0, capi.MODE_BLOCK)
@@ -190,8 +198,18 @@ def test_sync_refine_vs_oracle(ctx, marked):
         for o in range(65):
             if ve[k][o] and abs(E[k][o] - m) > best_v:
                 best_o, best_v = o, abs(E[k][o] - m)
-        assert int(unsorted[k]["index"]) == start + 8 * best_o, (k, int(unsorted[k]["index"]), start + 8 * best_o)
-        assert abs(abs(unsorted[k]["raw_quality"] - m) - best_v) < 1e-12
+        assert int(unsorted[k]["index"]) == start + 8 * best_o, (channels, k, int(unsorted[k]["index"]), start + 8 * best_o)
+        assert abs(abs(unsorted[k]["raw_quality"] - m) - best_v) < 1e-12, (channels, k)
+    # the exact per-offset qualities are the reference's sync_decode (sync_fft (fine)) on every offset of the best candidates and of
+    # the one whose window runs past the end
+    d = []
+    for k in (0, 1, 2, len(sel) - 1):
+        for o, (fine, q) in enumerate(sf.refine_qualities(y, O.BLOCK, sel[k].index, sb, KEY)):
+            assert ve[k][o] == (q is not None), (channels, k, o)
+            if q is not None:
+                d.append(abs(E[k][o] - q))
+    assert len(d) > 3 * 65 and max(d) < 2e-4, (channels, max(d))
+    print("channels %d: max |E - oracle| over %d offsets = %.3g" % (channels, len(d), max(d)))
 
 
 def test_decode_blocks_vs_oracle(ctx, marked):
