@@ -32,7 +32,7 @@ EXPORTS = [
     "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_approx_enqueue", "awm_sync_use_slot", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_sync_refine_rescored", "awm_decode_blocks", "awm_viterbi",
     "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_is_device_pointer", "awm_speed_scan", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_prefetch_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
     "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch", "awm_batch_rates_validate", "awm_embed_batch_rates",
-    "awm_batch_offsets_validate", "awm_embed_batch_offsets",
+    "awm_batch_offsets_validate", "awm_embed_batch_offsets", "awm_batch_rates_offsets_validate", "awm_embed_batch_rates_offsets",
 ]
 
 _lib = None
@@ -100,6 +100,22 @@ def batch_offsets_validate(items, n_values: int, zero_frames, sample_rate: int =
     err = ctypes.create_string_buffer(256)
     rc = load().awm_batch_offsets_validate(_ptr(it), ctypes.c_size_t(len(it)), ctypes.c_size_t(n_values), _ptr(zf), ctypes.c_int(sample_rate),
                                            ctypes.c_int(mark_sample_rate), err, ctypes.c_size_t(len(err)))
+    return err.value.decode() if rc else ""
+
+
+def batch_rates_offsets_validate(items, n_values: int, sample_rates, zero_frames, n_emit=None, mark_sample_rate: int = 44100) -> str:
+    """awm_batch_rates_offsets_validate: '' if awm_batch_rates_validate accepts the items and rates and every stream offset (frames at
+    the item's rate) is acceptable, else the reason"""
+    it = np.array([tuple(int(v) for v in t) for t in items], BATCH_ITEM)
+    rates = np.ascontiguousarray(sample_rates, np.int32)
+    emit = None if n_emit is None else np.ascontiguousarray(n_emit, np.uint64)
+    z = list(zero_frames)
+    if len(z) != len(it):
+        return "%d items but %d zero_frames" % (len(it), len(z))
+    zf = np.array([int(v) for v in z], np.uint64)
+    err = ctypes.create_string_buffer(256)
+    rc = load().awm_batch_rates_offsets_validate(_ptr(it), ctypes.c_size_t(len(it)), ctypes.c_size_t(n_values), _ptr(rates), _ptr(emit),
+                                                 _ptr(zf), ctypes.c_int(mark_sample_rate), err, ctypes.c_size_t(len(err)))
     return err.value.decode() if rc else ""
 
 

@@ -2629,11 +2629,35 @@ awm_batch_rates_validate (const awm_batch_item *items, size_t n_items, size_t n_
   return why[0] ? 1 : 0;
 }
 
+int
+awm_batch_rates_offsets_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const int *sample_rates, const uint64_t *n_emit,
+                                  const uint64_t *zero_frames, int mark_sample_rate, char *err, size_t err_cap)
+{
+  if (awm_batch_rates_validate (items, n_items, n_values, sample_rates, n_emit, mark_sample_rate, err, err_cap) ||
+      batch_offsets_check (items, n_items, n_values, zero_frames, true, err, err_cap))
+    return 1;
+  /* the stream at the watermark rate, (z + n) * mark / rate frames, must fit the limit too (at 8 kHz it is 5.5 times longer) */
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const unsigned __int128 end = (unsigned __int128) (zero_frames[i] + items[i].n_frames);
+      if (end * unsigned (mark_sample_rate) > (unsigned __int128) AWM_MAX_STREAM_FRAMES * unsigned (sample_rates[i]))
+        {
+          if (err && err_cap)
+            snprintf (err, err_cap, "batch item %zu: zero_frames %llu + n_frames %llu at %d Hz exceeds the stream length limit of 2^48 frames at %d Hz",
+                      i, (unsigned long long) zero_frames[i], (unsigned long long) items[i].n_frames, sample_rates[i], mark_sample_rate);
+          return 1;
+        }
+    }
+  if (err && err_cap)
+    err[0] = 0;
+  return 0;
+}
+
 namespace {
 
-/* awm_embed_batch, awm_embed_batch_offsets and awm_embed_batch_rates after their own argument checks (name: the error prefix).
- * sample_rates NULL: every item is at mark_sample_rate; zero_frames NULL: every item starts a stream.  Items at mark_sample_rate
- * use limiter_block44, the others rate * limiter_ms / 1000. */
+/* awm_embed_batch, awm_embed_batch_offsets, awm_embed_batch_rates and awm_embed_batch_rates_offsets after their own argument checks
+ * (name: the error prefix).  sample_rates NULL: every item is at mark_sample_rate; zero_frames NULL: every item starts a stream.
+ * Items at mark_sample_rate use limiter_block44, the others rate * limiter_ms / 1000; n_emit[i] counts from the item's first frame. */
 int
 embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
              const uint8_t *coded_bits, const uint64_t *zero_frames, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate,
@@ -2710,9 +2734,32 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
       R.h_out = f.h_out;
       R.coef_in = f.coef_in;
       R.coef_out = f.coef_out;
-      R.n44 = resampled_n44 (n_emit[i], R.step_out, R.h_out);
       R.limiter_block = block_of (rate);
-      R.n_blocks = R.limiter_block > 0 ? (R.n_emit + R.limiter_block - 1) / R.limiter_block + 1 : 0;   // every block the mixer reaches
+      if (zero_frames && zero_frames[i])
+        {
+          /* the stream of this item ends at z + n_emit, its x44 at n44 of that.  Everything before the first input frame the
+           * in-resampler's taps reach is silent: x44 is exactly +0 up to about (z - h_in) / step_in, the watermark up to one
+           * 1024-frame before that (the synthesis spill), so the scratch may start at w_hi or earlier.  It starts `span` frames
+           * before the end, a length that holds [w_hi, n44) for every z (bounds taken 16 frames early, rounding included): the
+           * scratch of an item does not depend on its offset.  The mixer starts where the out-resampler's taps reach w0. */
+          const long long z = (long long) zero_frames[i], end = z + R.n_emit;
+          const long long x_lo = std::max (0LL, (long long) floor (double (z - R.h_in - 16) / R.step_in));
+          const long long w_hi = std::max (x_lo / kFrame - 1, 0LL) * kFrame;
+          const long long n44 = resampled_n44 (uint64_t (end), R.step_out, R.h_out);
+          const long long span = ((long long) ceil ((double (R.n_emit + R.h_in + 32) * R.step_out + R.h_out) / kFrame) + 4) * kFrame;
+          R.z = z;
+          R.w0 = std::max (0LL, std::min (w_hi, n44 - span));
+          R.i0 = std::min (z, std::max (0LL, (long long) floor (double (R.w0 - R.h_out - 16) / R.step_out)));
+          R.blk0 = R.limiter_block > 0 ? R.i0 / R.limiter_block : 0;
+          R.n44 = n44 - R.w0;
+          R.n_emit = end - R.i0;
+          R.n_blocks = R.limiter_block > 0 ? (end - 1) / R.limiter_block - R.blk0 + 2 : 0;   // every block the mixer reaches
+        }
+      else
+        {
+          R.n44 = resampled_n44 (n_emit[i], R.step_out, R.h_out);
+          R.n_blocks = R.limiter_block > 0 ? (R.n_emit + R.limiter_block - 1) / R.limiter_block + 1 : 0;   // every block the mixer reaches
+        }
       R.peak0 = n_peaks;
       n_peaks += R.n_blocks;
       const size_t values = size_t (R.n44) * size_t (R.C);
@@ -2732,7 +2779,7 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
       if (R.limiter_block > 0)
         w.n_lim += (R.n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter);
       /* WatermarkGen::run on every 1024-frame of the scratch copy (src/wmadd.cc:394-399): n_frames = n44, no limiter, no --snr */
-      blist.push_back (batch_entry ((long long) w.values, R.n44, R.C, int (i), 0, w.n_tiles, unused, unused));
+      blist.push_back (batch_entry ((long long) w.values, R.n44, R.C, int (i), 0, w.n_tiles, unused, unused, R.w0));
       soff.push_back (w.values);
       w.values += values;
       rlist.push_back (R);
@@ -2785,18 +2832,23 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
           const RateItem *d_r = ctx->rate_items.as<RateItem>() + w.r0;
           const int n_r = int (w.r1 - w.r0);
           float *x44 = ctx->rate_scratch.as<float>();
+          /* items at stream offsets take their own instances, as k_embed_batch<true> does */
+          const bool offsets = zero_frames != nullptr;
           PROF (ctx);
-          k_resample_batch<<<unsigned (w.n_rs), kRateCta, 0, ctx->stream>>> (d_r, n_r);
+          (offsets ? k_resample_batch<true> : k_resample_batch<false>)<<<unsigned (w.n_rs), kRateCta, 0, ctx->stream>>> (d_r, n_r);
           LAUNCH_CHECK ("k_resample_batch");
-          if (launch_embed_batch (ctx, x44, x44 + w.values, d_b + w.b0, n_r, w.n_tiles, 0, frames_pad_start, water_delta, 0, limiter_ceiling, nullptr, 1))
+          if (launch_embed_batch (ctx, x44, x44 + w.values, d_b + w.b0, n_r, w.n_tiles, 0, frames_pad_start, water_delta, 0, limiter_ceiling, nullptr, 1,
+                                  offsets))
             return 1;
           PROF (ctx);
-          k_resample_mix_batch<<<unsigned (w.n_mix), kRateCta, 0, ctx->stream>>> (d_r, n_r, limiter_ceiling, ctx->peaks.as<unsigned>(), d_snr);
+          (offsets ? k_resample_mix_batch<true> : k_resample_mix_batch<false>)<<<unsigned (w.n_mix), kRateCta, 0, ctx->stream>>> (
+            d_r, n_r, limiter_ceiling, ctx->peaks.as<unsigned>(), d_snr);
           LAUNCH_CHECK ("k_resample_mix_batch");
           if (w.n_lim)
             {
               PROF (ctx);
-              k_limiter_rates<<<unsigned (w.n_lim), 256, 0, ctx->stream>>> (d_r, n_r, limiter_ceiling, ctx->peaks.as<unsigned>());
+              (offsets ? k_limiter_rates<true> : k_limiter_rates<false>)<<<unsigned (w.n_lim), 256, 0, ctx->stream>>> (
+                d_r, n_r, limiter_ceiling, ctx->peaks.as<unsigned>());
               LAUNCH_CHECK ("k_limiter_rates");
             }
         }
@@ -2842,6 +2894,20 @@ awm_embed_batch_rates (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, 
     return fail (ctx, "awm_embed_batch_rates: %s", why);
   return embed_batch ("awm_embed_batch_rates", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, nullptr, sample_rates, n_emit,
                       mark_sample_rate, frames_pad_start, water_delta, int ((long long) mark_sample_rate * limiter_ms / 1000), limiter_ms,
+                      limiter_ceiling, snr_power, scratch_bytes);
+}
+
+int
+awm_embed_batch_rates_offsets (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                               const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, const uint64_t *zero_frames,
+                               int mark_sample_rate, int frames_pad_start, double water_delta, int limiter_ms, float limiter_ceiling,
+                               double *snr_power, size_t scratch_bytes)
+{
+  char why[240];
+  if (awm_batch_rates_offsets_validate (items, n_items, n_values, sample_rates, n_emit, zero_frames, mark_sample_rate, why, sizeof (why)))
+    return fail (ctx, "awm_embed_batch_rates_offsets: %s", why);
+  return embed_batch ("awm_embed_batch_rates_offsets", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, zero_frames, sample_rates,
+                      n_emit, mark_sample_rate, frames_pad_start, water_delta, int ((long long) mark_sample_rate * limiter_ms / 1000), limiter_ms,
                       limiter_ceiling, snr_power, scratch_bytes);
 }
 

@@ -40,21 +40,39 @@ resampled_add_plan (size_t n_frames, int sample_rate, bool limiter_on, size_t li
 {
   const size_t N = Params::frame_size;
   const double r_in = double (Params::mark_sample_rate) / sample_rate, r_out = double (sample_rate) / Params::mark_sample_rate;
-  size_t total_in = 0, total_out = 0;
-  n_emit = gen_runs_out = 0;
-  for (size_t iteration = 1;; iteration++)
+  /* the state after `iteration` blocks were pushed; released (frames the limiter has let out) never decreases */
+  auto state = [&] (size_t iteration, size_t& emit, size_t& runs)
     {
-      const size_t real = std::min (N, n_frames - total_in);
-      total_in += real;
-      if (real < N && total_in == total_out)
-        break;
-      const size_t at_mark_rate = resample_stream_available (N * iteration, r_in);
-      gen_runs_out = at_mark_rate / N;
-      n_emit = gen_runs_out ? resample_stream_available (gen_runs_out * N, r_out) : 0;
-      size_t released = n_emit;
-      if (limiter_on)
-        released = n_emit / limiter_block >= 2 ? (n_emit / limiter_block - 1) * limiter_block : 0;
-      total_out = std::min (released, total_in);
+      runs = resample_stream_available (N * iteration, r_in) / N;
+      emit = runs ? resample_stream_available (runs * N, r_out) : 0;
+      if (!limiter_on)
+        return emit;
+      return emit / limiter_block >= 2 ? (emit / limiter_block - 1) * limiter_block : 0;
+    };
+  n_emit = gen_runs_out = 0;
+  if (n_frames == 0)
+    return;
+  /* the loop stops after the first iteration k that has read all input (N k >= n_frames) and released all of it: the first k
+   * at or after ceil (n_frames / N) with released (k) >= n_frames, found by doubling the step and then bisecting */
+  size_t lo = (n_frames + N - 1) / N;
+  if (state (lo, n_emit, gen_runs_out) < n_frames)
+    {
+      size_t step = 1, hi;
+      while (state (lo + step, n_emit, gen_runs_out) < n_frames)
+        {
+          lo += step;
+          step *= 2;
+        }
+      hi = lo + step;                 /* released (lo) < n_frames <= released (hi) */
+      while (hi - lo > 1)
+        {
+          const size_t mid = lo + (hi - lo) / 2;
+          if (state (mid, n_emit, gen_runs_out) < n_frames)
+            lo = mid;
+          else
+            hi = mid;
+        }
+      state (hi, n_emit, gen_runs_out);
     }
 }
 
@@ -208,10 +226,12 @@ add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t
 
 int
 add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                           const vector<string>& bits, const int *sample_rates, size_t scratch_bytes, vector<AddStats> *stats)
+                           const vector<string>& bits, const int *sample_rates, size_t scratch_bytes, vector<AddStats> *stats,
+                           const uint64_t *zero_frames)
 {
   char why[256];
-  if (awm_batch_rates_validate (items, n_items, n_values, sample_rates, nullptr, Params::mark_sample_rate, why, sizeof (why)))
+  if (zero_frames ? awm_batch_rates_offsets_validate (items, n_items, n_values, sample_rates, nullptr, zero_frames, Params::mark_sample_rate, why, sizeof (why))
+                  : awm_batch_rates_validate (items, n_items, n_values, sample_rates, nullptr, Params::mark_sample_rate, why, sizeof (why)))
     {
       error ("audiowmark: %s\n", why);
       return 2;
@@ -225,29 +245,37 @@ add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, 
       const vector<uint8_t> c = gen_coded_bits (key, bitvec);
       coded.insert (coded.end(), c.begin(), c.end());
     }
-  /* per item what add_watermark_buffer computes for it: frames through the mixer (other rates) and WatermarkGen::run calls */
+  /* per item what add_watermark_buffer computes for its whole stream (silent prefix included, as add_watermark_windowed counts):
+   * frames through the mixer (other rates; counted from the item's first frame) and WatermarkGen::run calls */
   vector<uint64_t> n_emit (n_items);
   vector<size_t> runs (n_items);
   for (size_t i = 0; i < n_items; i++)
     {
       const int rate = sample_rates[i];
       const size_t block = size_t (rate) * size_t (Params::limiter_block_size_ms) / 1000;
+      const size_t z = zero_frames ? zero_frames[i] : 0, n_stream = z + items[i].n_frames;
       if (rate == Params::mark_sample_rate)
         {
-          runs[i] = gen_runs (items[i].n_frames, !Params::test_no_limiter, block);
+          runs[i] = gen_runs (n_stream, !Params::test_no_limiter, block);
           continue;
         }
       size_t emit = 0;
-      resampled_add_plan (items[i].n_frames, rate, !Params::test_no_limiter, block, emit, runs[i]);
-      n_emit[i] = std::max<uint64_t> (emit, items[i].n_frames);
+      resampled_add_plan (n_stream, rate, !Params::test_no_limiter, block, emit, runs[i]);
+      n_emit[i] = std::max<uint64_t> (emit, n_stream) - z;
     }
   awm_ctx *ctx = Engine::ctx();
   if (!ctx || !Engine::set_embed_roles (key))
     return 1;
   vector<double> snr_power (2 * n_items);
-  if (awm_embed_batch_rates (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), Params::mark_sample_rate,
-                             Params::frames_pad_start, Params::water_delta, Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms),
-                             Params::limiter_ceiling, (Params::snr || stats) ? snr_power.data() : nullptr, scratch_bytes))
+  const int limiter_ms = Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms);
+  double *snr = (Params::snr || stats) ? snr_power.data() : nullptr;
+  const int rc = zero_frames
+    ? awm_embed_batch_rates_offsets (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), zero_frames,
+                                     Params::mark_sample_rate, Params::frames_pad_start, Params::water_delta, limiter_ms, Params::limiter_ceiling, snr,
+                                     scratch_bytes)
+    : awm_embed_batch_rates (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), Params::mark_sample_rate,
+                             Params::frames_pad_start, Params::water_delta, limiter_ms, Params::limiter_ceiling, snr, scratch_bytes);
+  if (rc)
     {
       error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
       return 1;

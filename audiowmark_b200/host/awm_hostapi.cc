@@ -316,14 +316,15 @@ awmh_add_batch_offsets_s16 (const unsigned char *key16, const int16_t *in, int16
 /* add_watermark_batch_rates on a packed buffer: items[i] is at sample_rates[i]; otherwise as awmh_add_batch */
 static int
 add_batch_rates_any (const unsigned char *key16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                     const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db)
+                     const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db,
+                     const uint64_t *zero_frames = nullptr)
 {
   std::vector<std::string> bits (n_items);
   for (size_t i = 0; i < n_items; i++)
     bits[i] = payload_hex[i] ? payload_hex[i] : "";
   std::vector<AddStats> stats;
   const int rc = add_watermark_batch_rates (make_key (key16, ""), in, out, s16, n_values, items, n_items, bits, sample_rates, scratch_bytes,
-                                            (data_blocks || snr_db) ? &stats : nullptr);
+                                            (data_blocks || snr_db) ? &stats : nullptr, zero_frames);
   for (size_t i = 0; i < stats.size(); i++)
     {
       if (data_blocks)
@@ -346,6 +347,27 @@ awmh_add_batch_rates_s16 (const unsigned char *key16, const int16_t *in, int16_t
                           const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db)
 {
   return add_batch_rates_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
+}
+
+/* add_watermark_batch_rates with stream offsets: items[i] continues a stream at sample_rates[i] that began zero_frames[i] frames (at
+ * that rate) earlier with silence (an HLS segment of a 48 kHz master); otherwise as awmh_add_batch_rates.  Returns 2 for a malformed
+ * offset list too (awm_batch_rates_offsets_validate). */
+int
+awmh_add_batch_rates_offsets (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                              const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes,
+                              int *data_blocks, double *snr_db)
+{
+  return add_batch_rates_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db,
+                              zero_frames);
+}
+
+int
+awmh_add_batch_rates_offsets_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items,
+                                  size_t n_items, const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates,
+                                  size_t scratch_bytes, int *data_blocks, double *snr_db)
+{
+  return add_batch_rates_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db,
+                              zero_frames);
 }
 
 /* add / get between 16 bit PCM host buffers (the contents of a 16 bit WAV file): conversions run on the device */

@@ -29,10 +29,13 @@ int add_watermark_batch (const Key& key, const void *in, void *out, bool s16, si
 
 /* add_watermark_batch for items that each have their own sample rate (sample_rates[i]): item i comes out bit identical to
  * add_watermark_buffer on it alone at that rate (16 bit items: converted to float and back around it, as `audiowmark add` does for a
- * 16 bit file).  scratch_bytes: awm_embed_batch_rates's wave size, 0 = its default.  Returns 2 for a malformed item list, rate or
- * payload, 1 for other errors. */
+ * 16 bit file).  scratch_bytes: awm_embed_batch_rates's wave size, 0 = its default.  zero_frames (optional, [n_items], frames at the
+ * item's own rate): item i continues a stream that began zero_frames[i] frames earlier with silence: it comes out as
+ * add_watermark_buffer of zeros (z) ++ item with the first z frames dropped, Data Blocks counted over that stream, --snr over the
+ * item's own positions.  Returns 2 for a malformed item list, rate, offset list or payload, 1 for other errors. */
 int add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                               const std::vector<std::string>& bits, const int *sample_rates, size_t scratch_bytes, std::vector<AddStats> *stats);
+                               const std::vector<std::string>& bits, const int *sample_rates, size_t scratch_bytes, std::vector<AddStats> *stats,
+                               const uint64_t *zero_frames = nullptr);
 
 /* add_stream_watermark's loop with bounded memory (window by window; see awm_add.cc); callbacks read / write interleaved frames */
 int add_watermark_windowed (const Key& key, const std::function<Error (std::vector<float>&, size_t)>& read,

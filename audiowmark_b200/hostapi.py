@@ -18,7 +18,7 @@ CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
            "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_add_windowed",
            "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16", "awmh_add_batch_rates", "awmh_add_batch_rates_s16",
-           "awmh_add_batch_offsets", "awmh_add_batch_offsets_s16"]
+           "awmh_add_batch_offsets", "awmh_add_batch_offsets_s16", "awmh_add_batch_rates_offsets", "awmh_add_batch_rates_offsets_s16"]
 
 _lib = None
 
@@ -264,12 +264,16 @@ def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None,
     return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs
 
 
-def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None, want_stats=False, scratch_bytes=0):
+def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None, want_stats=False, scratch_bytes=0, zero_frames=None):
     """add_batch for items that each have their own sample rate: item i comes out bit identical to add(item, payloads[i],
     sample_rate=sample_rates[i]) of that item alone (16 bit items: to that `add` between int16_to_float and 16 bit quantisation, what
     `audiowmark add` computes on a 16 bit file).  pcms / items / out / want_stats as in add_batch.  scratch_bytes: device scratch
     per wave of resampled items (0: the library's default of 4 GiB; a smaller value runs more, smaller waves with the same result).
-    Raises ValueError for a malformed item list, rate list or payload."""
+    zero_frames: None, or one stream offset per item in frames at that item's rate: item i continues a stream that began
+    zero_frames[i] frames earlier with silence (an HLS segment of a 48 kHz master).  It comes out bit identical to
+    add_batch_rates([zeros(z) ++ item], ...)[z:], with the data blocks of that whole stream and the SNR of the item's own positions;
+    the silent prefix is never allocated.  zero_frames + n_frames is limited to 2^48 per item, at the item's rate and at 44.1 kHz.
+    Raises ValueError for a malformed item list, rate list, offset list or payload."""
     payloads = list(payloads)
     rates = np.array([int(r) for r in sample_rates], np.int64)
     s16, it, n_values, p_in, p_out, split, _keep = _pack_batch("add_batch_rates", pcms, payloads, items, out)
@@ -278,14 +282,21 @@ def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None
     if np.any(rates <= 0) or np.any(rates > np.iinfo(np.int32).max):
         raise ValueError("add_batch_rates: sample rates must be positive 32 bit integers")
     rates = np.ascontiguousarray(rates, np.int32)
+    z = None if zero_frames is None else _zero_frames("add_batch_rates", zero_frames, len(it))
     pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
     blocks = np.zeros(max(len(it), 1), np.int32)
     snr = np.zeros(max(len(it), 1), np.float64)
-    fn = load().awmh_add_batch_rates_s16 if s16 else load().awmh_add_batch_rates
-    rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, _ptr(rates),
-            ctypes.c_size_t(scratch_bytes), _ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
+    stats = (_ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
+    if z is None:
+        fn = load().awmh_add_batch_rates_s16 if s16 else load().awmh_add_batch_rates
+        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, _ptr(rates),
+                ctypes.c_size_t(scratch_bytes), *stats)
+    else:
+        fn = load().awmh_add_batch_rates_offsets_s16 if s16 else load().awmh_add_batch_rates_offsets
+        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), _ptr(z), pay, _ptr(rates),
+                ctypes.c_size_t(scratch_bytes), *stats)
     if rc == 2:
-        raise ValueError("add_batch_rates: malformed item list, sample rate or payload; see stderr")
+        raise ValueError("add_batch_rates: malformed item list, sample rate, offset list or payload; see stderr")
     if rc:
         raise RuntimeError("awmh_add_batch_rates failed (rc=%d); see stderr" % rc)
     synchronize()

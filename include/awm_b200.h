@@ -225,6 +225,23 @@ int awm_batch_rates_validate (const awm_batch_item *items, size_t n_items, size_
 int awm_embed_batch_rates (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
                            const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate, int frames_pad_start,
                            double water_delta, int limiter_ms, float limiter_ceiling, double *snr_power, size_t scratch_bytes);
+/* 0 if awm_batch_rates_validate passes, zero_frames is not NULL (for n_items > 0) and every item's stream, zero_frames[i] +
+ * n_frames, is at most AWM_MAX_STREAM_FRAMES both at sample_rates[i] and at mark_sample_rate ((z + n) * mark / rate); else nonzero
+ * with the reason in err.  Needs no device. */
+int awm_batch_rates_offsets_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const int *sample_rates, const uint64_t *n_emit,
+                                      const uint64_t *zero_frames, int mark_sample_rate, char *err, size_t err_cap);
+/* awm_embed_batch_rates for items that are segments of longer streams at any sample rate (HLS segments of a 48 kHz master:
+ * add_stream_watermark with zero_frames, src/wmadd.cc:501-580).  Item i continues a stream at sample_rates[i] that began
+ * zero_frames[i] frames (at that rate) earlier with silence: it comes out bit identical to item 0 of awm_embed_batch_rates on
+ * zeros (zero_frames[i]) ++ item, with the first zero_frames[i] frames dropped.  Both resamplers, the watermark frames and the
+ * limiter blocks are those of that stream; the silent prefix is never allocated, read or resampled, and an item's scratch does not
+ * grow with its offset.  n_emit[i] counts from the item's first frame: the whole stream's n_emit minus zero_frames[i].  snr_power[i]
+ * sums the item's own positions [z, z + n_emit[i]) only.  Items at mark_sample_rate are those of awm_embed_batch_offsets.  All
+ * offsets zero gives exactly awm_embed_batch_rates; every rate at mark_sample_rate gives exactly awm_embed_batch_offsets. */
+int awm_embed_batch_rates_offsets (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                                   const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, const uint64_t *zero_frames,
+                                   int mark_sample_rate, int frames_pad_start, double water_delta, int limiter_ms, float limiter_ceiling,
+                                   double *snr_power, size_t scratch_bytes);
 
 /* ---- sync search on the bound PCM --------------------------------------------------------
  * awm_sync_approx = SyncFinder::search_approx (src/syncfinder.cc:171-256): for the four
