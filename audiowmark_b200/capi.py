@@ -33,6 +33,7 @@ EXPORTS = [
     "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_is_device_pointer", "awm_speed_scan", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_prefetch_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
     "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch", "awm_batch_rates_validate", "awm_embed_batch_rates",
     "awm_batch_offsets_validate", "awm_embed_batch_offsets", "awm_batch_rates_offsets_validate", "awm_embed_batch_rates_offsets",
+    "awm_set_embed_roles_keys", "awm_get_embed_roles_keys", "awm_batch_keys_validate", "awm_embed_batch_keys",
 ]
 
 _lib = None
@@ -119,6 +120,24 @@ def batch_rates_offsets_validate(items, n_values: int, sample_rates, zero_frames
     return err.value.decode() if rc else ""
 
 
+def batch_keys_validate(items, n_values: int, key_index, n_keys: int, sample_rates=None, zero_frames=None, n_emit=None,
+                        mark_sample_rate: int = 44100) -> str:
+    """awm_batch_keys_validate: '' if the checks of the matching single-key validator pass and every key index (None: a NULL list) is
+    below n_keys, else the reason"""
+    it = np.array([tuple(int(v) for v in t) for t in items], BATCH_ITEM)
+    rates = None if sample_rates is None else np.ascontiguousarray(sample_rates, np.int32)
+    emit = None if n_emit is None else np.ascontiguousarray(n_emit, np.uint64)
+    zf = None if zero_frames is None else np.array([int(v) for v in zero_frames], np.uint64)
+    ki = None if key_index is None else np.array([int(v) for v in key_index], np.uint32)
+    for name, arr in (("sample_rates", rates), ("zero_frames", zf), ("key_index", ki)):
+        if arr is not None and len(arr) != len(it):
+            return "%d items but %d %s" % (len(it), len(arr), name)
+    err = ctypes.create_string_buffer(256)
+    rc = load().awm_batch_keys_validate(_ptr(it), ctypes.c_size_t(len(it)), ctypes.c_size_t(n_values), _ptr(rates), _ptr(emit), _ptr(zf), _ptr(ki),
+                                        ctypes.c_size_t(n_keys), ctypes.c_int(mark_sample_rate), err, ctypes.c_size_t(len(err)))
+    return err.value.decode() if rc else ""
+
+
 class Context:
     """One awm_ctx (device + stream)."""
 
@@ -190,6 +209,19 @@ class Context:
         fm = np.ascontiguousarray(frame_mod_ab, np.uint8)
         assert fm.ndim == 3 and fm.shape[0] == 2 and fm.shape[2] == 101
         self._ck(self.lib.awm_set_embed_tables(self.h, _ptr(fm), ctypes.c_int(fm.shape[1])))
+
+    def set_embed_roles_keys(self, keys, layout):
+        """awm_set_embed_roles_keys: build the role tables of keys (16-byte keys, or a uint8 array [n, 16]) on the device; layout: the 6
+        ints of awm_role_layout (hostapi.role_layout())"""
+        kb = np.ascontiguousarray(np.frombuffer(b"".join(bytes(k) for k in keys), np.uint8) if not isinstance(keys, np.ndarray) else keys, np.uint8)
+        lay = np.ascontiguousarray(layout, np.int32)
+        assert kb.size % 16 == 0 and lay.shape == (6,)
+        self._ck(self.lib.awm_set_embed_roles_keys(self.h, _ptr(kb), ctypes.c_size_t(kb.size // 16), _ptr(lay)))
+
+    def get_embed_roles_keys(self, first_key: int, n_keys: int, frames_per_block: int) -> np.ndarray:
+        out = np.zeros((n_keys, frames_per_block, 101), np.uint16)
+        self._ck(self.lib.awm_get_embed_roles_keys(self.h, ctypes.c_size_t(first_key), ctypes.c_size_t(n_keys), _ptr(out)))
+        return out
 
     def set_sync_tables(self, key_slot: int, mode: int, entries: np.ndarray, bit_offsets: np.ndarray):
         e = np.ascontiguousarray(entries, SYNC_ENTRY)

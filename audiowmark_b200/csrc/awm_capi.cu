@@ -14,6 +14,7 @@
 #include "awm_embed_strip.cuh"
 #include "awm_embed_batch.cuh"
 #include "awm_batch_rates.cuh"
+#include "awm_keygen.cuh"
 
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -150,6 +151,10 @@ struct awm_ctx
   DevBuf frame_mod; int embed_fpb = 0;
   DevBuf roles; int roles_fpb = 0, roles_n_coded = 0;         // batched embed: role table of one key
   DevBuf batch_items, batch_coded;
+  /* batched embed with a key per item: role tables of n_keys keys built on the device (awm_set_embed_roles_keys) and the builder's
+   * scratch (j values, bands of the data entries, index array of a mix too large for shared memory, per-key error flags) */
+  DevBuf key_roles, keygen_keys, keygen_j, keygen_ud, keygen_idx, keygen_err;
+  size_t key_roles_n = 0; int key_roles_fpb = 0, key_roles_n_coded = 0;
   DevBuf rate_items, rate_scratch;                           // batched embed at other sample rates: work list, per-wave scratch
   KeyTab keys[AWM_MAX_KEYS];
 
@@ -378,7 +383,7 @@ awm_destroy (awm_ctx *ctx)
   cudaStreamSynchronize (ctx->stream);
   if (ctx->s_approx)
     cudaStreamSynchronize (ctx->s_approx);
-  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->rate_items, &ctx->rate_scratch, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
+  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->key_roles, &ctx->keygen_keys, &ctx->keygen_j, &ctx->keygen_ud, &ctx->keygen_idx, &ctx->keygen_err, &ctx->rate_items, &ctx->rate_scratch, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
                      &ctx->cand_start, &ctx->cand_noff, &ctx->r_ud, &ctx->r_cnt, &ctx->rvalid, &ctx->r_ent_ud, &ctx->r_ent_flag, &ctx->tw1024,
                      &ctx->cand_score, &ctx->rank_keep, &ctx->rank_first, &ctx->ex_start, &ctx->ex_cand, &ctx->ex_off, &ctx->ex_n, &ctx->vit_off, &ctx->blk_start, &ctx->D, &ctx->raw,
                      &ctx->vit_raw, &ctx->vit_types, &ctx->vit_delta, &ctx->vit_dec, &ctx->vit_bits, &ctx->vit_err,
@@ -612,6 +617,76 @@ awm_set_embed_roles (awm_ctx *ctx, const uint16_t *roles, int frames_per_block, 
   CK (cudaStreamSynchronize (ctx->stream));
   ctx->roles_fpb = frames_per_block;
   ctx->roles_n_coded = n_coded_bits;
+  return 0;
+}
+
+int
+awm_set_embed_roles_keys (awm_ctx *ctx, const uint8_t *keys16, size_t n_keys, const awm_role_layout *layout)
+{
+  ctx->key_roles_n = 0;
+  if (!keys16 || !n_keys || n_keys > INT_MAX || !layout)
+    return fail (ctx, "awm_set_embed_roles_keys: bad arguments");
+  const awm_role_layout& l = *layout;
+  if (l.sync_frames <= 0 || l.sync_frames_per_bit <= 0 || l.sync_frames % l.sync_frames_per_bit || l.frames_per_bit <= 0 || l.n_coded_bits <= 0 ||
+      l.n_coded_bits > AWM_ROLE_MAX_INDEX + 1 || l.sync_frames / l.sync_frames_per_bit > AWM_ROLE_MAX_INDEX + 1 ||
+      (long long) l.n_coded_bits * l.frames_per_bit != l.data_frames || (long long) l.sync_frames + l.data_frames > 65536)
+    return fail (ctx, "awm_set_embed_roles_keys: bad layout (sync frames %d, %d per bit, data frames %d, %d per bit, %d coded bits)",
+                 l.sync_frames, l.sync_frames_per_bit, l.data_frames, l.frames_per_bit, l.n_coded_bits);
+  KeygenLayout L;
+  L.sync_frames = l.sync_frames;
+  L.sync_frames_per_bit = l.sync_frames_per_bit;
+  L.data_frames = l.data_frames;
+  L.frames_per_bit = l.frames_per_bit;
+  L.mix = l.mix != 0;
+  L.fpb = l.sync_frames + l.data_frames;
+  L.n_mix = l.data_frames * AWM_BANDS_PER_FRAME;
+  L.j_mix0 = (L.fpb + 15) & ~15;
+  L.j_stride = L.j_mix0 + (L.mix ? (L.n_mix + 15) & ~15 : 0);
+  const bool smem_idx = !L.mix || L.n_mix <= kKeygenSmemIdxMax;      /* a larger mix keeps its index array in global memory */
+  const size_t smem = keygen_smem (L.fpb, L.n_mix, L.mix && smem_idx);
+  CK (cudaSetDevice (ctx->device));
+  int smem_max = 0;
+  CK (cudaDeviceGetAttribute (&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+  if (smem > size_t (smem_max))
+    return fail (ctx, "awm_set_embed_roles_keys: %d frames per block need %zu bytes of shared memory (%d available)", L.fpb, smem, smem_max);
+  const size_t n_roles = n_keys * size_t (L.fpb) * (kMaxBand + 1);
+  CK (ctx->key_roles.reserve (n_roles * sizeof (uint16_t)));
+  CK (ctx->keygen_keys.reserve (n_keys * 16));
+  CK (ctx->keygen_j.reserve (n_keys * size_t (L.j_stride) * sizeof (uint32_t)));
+  CK (ctx->keygen_ud.reserve (L.mix ? n_keys * 2 * size_t (L.n_mix) : 16));
+  CK (ctx->keygen_idx.reserve (L.mix && !smem_idx ? n_keys * size_t (L.n_mix) * sizeof (uint32_t) : 16));
+  CK (ctx->keygen_err.reserve (n_keys * sizeof (int)));
+  CK (cudaMemcpyAsync (ctx->keygen_keys.p, keys16, n_keys * 16, cudaMemcpyDefault, ctx->stream));
+  CK (cudaMemsetAsync (ctx->keygen_err.p, 0, n_keys * sizeof (int), ctx->stream));
+  auto kernel = smem_idx ? k_embed_roles_keys<true> : k_embed_roles_keys<false>;
+  if (set_smem (ctx, kernel, smem)) return 1;
+  PROF (ctx);
+  kernel<<<unsigned (n_keys), kKeygenThreads, smem, ctx->stream>>> (ctx->keygen_keys.as<uint8_t>(), L, ctx->key_roles.as<uint16_t>(), ctx->keygen_j.as<uint32_t>(),
+                                                                    ctx->keygen_ud.as<uint8_t>(), ctx->keygen_idx.as<uint32_t>(), ctx->keygen_err.as<int>());
+  LAUNCH_CHECK ("k_embed_roles_keys");
+  std::vector<int> errs (n_keys);
+  CK (cudaMemcpyAsync (errs.data(), ctx->keygen_err.p, n_keys * sizeof (int), cudaMemcpyDeviceToHost, ctx->stream));
+  CK (cudaStreamSynchronize (ctx->stream));
+  for (size_t k = 0; k < n_keys; k++)
+    if (errs[k])
+      return fail (ctx, "awm_set_embed_roles_keys: key %zu: a (frame, bin) entry is assigned twice", k);
+  ctx->key_roles_n = n_keys;
+  ctx->key_roles_fpb = L.fpb;
+  ctx->key_roles_n_coded = l.n_coded_bits;
+  return 0;
+}
+
+int
+awm_get_embed_roles_keys (awm_ctx *ctx, size_t first_key, size_t n_keys, uint16_t *out)
+{
+  if (first_key > ctx->key_roles_n || n_keys > ctx->key_roles_n - first_key || (n_keys && !out))
+    return fail (ctx, "awm_get_embed_roles_keys: keys %zu .. %zu of a role set of %zu keys", first_key, first_key + n_keys, ctx->key_roles_n);
+  if (!n_keys)
+    return 0;
+  CK (cudaSetDevice (ctx->device));
+  const size_t per_key = size_t (ctx->key_roles_fpb) * (kMaxBand + 1);
+  CK (cudaMemcpyAsync (out, ctx->key_roles.as<uint16_t>() + first_key * per_key, n_keys * per_key * sizeof (uint16_t), cudaMemcpyDefault, ctx->stream));
+  CK (cudaStreamSynchronize (ctx->stream));
   return 0;
 }
 
@@ -1356,9 +1431,10 @@ batch_finish (awm_ctx *ctx, void *out_v, bool s16, size_t n_values, const float 
  * frame (awm_embed_batch.cuh) */
 BatchItem
 batch_entry (long long v0, long long n_frames, int C, int item, int limiter_block, long long& n_tiles, long long& n_lim, long long& n_peaks,
-             long long zero_frames = 0)
+             long long zero_frames = 0, int role_table = 0)
 {
   BatchItem b;
+  b.role_table = role_table;
   b.v0 = v0;
   b.n_frames = n_frames;
   b.C = C;
@@ -1377,17 +1453,20 @@ batch_entry (long long v0, long long n_frames, int C, int item, int limiter_bloc
   return b;
 }
 
+/* the role tables a batch reads: one key's (awm_set_embed_roles) or a key set's (awm_set_embed_roles_keys), [role_table][fpb][101] */
+struct RoleSet { const uint16_t *p; int fpb, n_coded; bool per_item; };
+
 /* k_embed_batch over the n_list items at d_items (v0 relative to in / out), then k_limiter_batch when limiter_block > 0.
  * Peaks go to ctx->peaks (zeroed by the caller), --snr sums to d_snr (null: none); delta_only: write the watermark signal alone */
 int
-launch_embed_batch (awm_ctx *ctx, const float *in, float *out, const BatchItem *d_items, int n_list, long long n_tiles, long long n_lim,
+launch_embed_batch (awm_ctx *ctx, const RoleSet& rs, const float *in, float *out, const BatchItem *d_items, int n_list, long long n_tiles, long long n_lim,
                     int frames_pad_start, double water_delta, int limiter_block, float limiter_ceiling, double *d_snr, int delta_only,
                     bool offsets = false)
 {
   EmbedArgs A = {};
   A.in = in;
   A.out = out;
-  A.fpb = ctx->roles_fpb;
+  A.fpb = rs.fpb;
   A.frame_number0 = 2LL * A.fpb - frames_pad_start;       // of a stream start; each item adds its frame0
   A.pow_up = 0.5f * float (-water_delta * 1);
   A.pow_down = 0.5f * float (-water_delta * -1);
@@ -1399,12 +1478,13 @@ launch_embed_batch (awm_ctx *ctx, const float *in, float *out, const BatchItem *
   A.tw = ctx->tw.as<float2>();
   A.win = ctx->win.as<float>();
   A.synth = ctx->synth.as<float>();
-  /* items at stream offsets take their own instance: the offset arithmetic costs the stream-start case registers and spills */
-  auto kernel = offsets ? k_embed_batch<true> : k_embed_batch<false>;
+  /* items at stream offsets take their own instance: the offset arithmetic costs the stream-start case registers and spills; so does
+   * a role table per item, whose batches always take the offsets instance (zero offsets give the stream-start result) */
+  auto kernel = rs.per_item ? k_embed_batch<true, true> : offsets ? k_embed_batch<true, false> : k_embed_batch<false, false>;
   if (set_smem (ctx, kernel, kEmbedBatchSmem)) return 1;
   PROF (ctx);
-  kernel<<<unsigned (n_tiles), kEmbedWarps * 32, kEmbedBatchSmem, ctx->stream>>> (A, d_items, n_list, ctx->roles.as<uint16_t>(),
-                                                                                 ctx->batch_coded.as<uint8_t>(), ctx->roles_n_coded);
+  kernel<<<unsigned (n_tiles), kEmbedWarps * 32, kEmbedBatchSmem, ctx->stream>>> (A, d_items, n_list, rs.p, ctx->batch_coded.as<uint8_t>(),
+                                                                                 rs.n_coded);
   LAUNCH_CHECK ("k_embed_batch");
   if (limiter_block > 0)
     {
@@ -2653,19 +2733,50 @@ awm_batch_rates_offsets_validate (const awm_batch_item *items, size_t n_items, s
   return 0;
 }
 
+int
+awm_batch_keys_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const int *sample_rates, const uint64_t *n_emit,
+                         const uint64_t *zero_frames, const uint32_t *key_index, size_t n_keys, int mark_sample_rate, char *err, size_t err_cap)
+{
+  if (sample_rates ? (zero_frames ? awm_batch_rates_offsets_validate (items, n_items, n_values, sample_rates, n_emit, zero_frames, mark_sample_rate, err, err_cap)
+                                  : awm_batch_rates_validate (items, n_items, n_values, sample_rates, n_emit, mark_sample_rate, err, err_cap))
+                   : batch_offsets_check (items, n_items, n_values, zero_frames, false, err, err_cap))
+    return 1;
+  char why[160] = "";
+  if (n_items && !key_index)
+    snprintf (why, sizeof (why), "key index list is NULL");
+  else if (n_items && !n_keys)
+    snprintf (why, sizeof (why), "the role set has no keys");
+  for (size_t i = 0; i < n_items && !why[0]; i++)
+    if (key_index[i] >= n_keys)
+      snprintf (why, sizeof (why), "batch item %zu: key index %u is out of range (%zu keys)", i, key_index[i], n_keys);
+  if (err && err_cap)
+    snprintf (err, err_cap, "%s", why);
+  return why[0] ? 1 : 0;
+}
+
 namespace {
 
-/* awm_embed_batch, awm_embed_batch_offsets, awm_embed_batch_rates and awm_embed_batch_rates_offsets after their own argument checks
- * (name: the error prefix).  sample_rates NULL: every item is at mark_sample_rate; zero_frames NULL: every item starts a stream.
- * Items at mark_sample_rate use limiter_block44, the others rate * limiter_ms / 1000; n_emit[i] counts from the item's first frame. */
+/* awm_embed_batch, awm_embed_batch_offsets, awm_embed_batch_rates, awm_embed_batch_rates_offsets and awm_embed_batch_keys after their
+ * own argument checks (name: the error prefix).  sample_rates NULL: every item is at mark_sample_rate; zero_frames NULL: every item
+ * starts a stream; key_index NULL: every item uses the role table of awm_set_embed_roles, else item i that of key key_index[i] of
+ * the role set of awm_set_embed_roles_keys.  Items at mark_sample_rate use limiter_block44, the others rate * limiter_ms / 1000;
+ * n_emit[i] counts from the item's first frame. */
 int
 embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
              const uint8_t *coded_bits, const uint64_t *zero_frames, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate,
              int frames_pad_start, double water_delta, int limiter_block44, int limiter_ms, float limiter_ceiling, double *snr_power,
-             size_t scratch_bytes)
+             size_t scratch_bytes, const uint32_t *key_index = nullptr)
 {
-  if (!ctx->roles_fpb)
+  RoleSet rs { ctx->roles.as<uint16_t>(), ctx->roles_fpb, ctx->roles_n_coded, false };
+  if (key_index)
+    {
+      if (!ctx->key_roles_n)
+        return fail (ctx, "%s: awm_set_embed_roles_keys has not been called", name);
+      rs = { ctx->key_roles.as<uint16_t>(), ctx->key_roles_fpb, ctx->key_roles_n_coded, true };
+    }
+  else if (!ctx->roles_fpb)
     return fail (ctx, "%s: awm_set_embed_roles has not been called", name);
+  auto role_table = [&] (size_t i) { return key_index ? int (key_index[i]) : 0; };
   if ((n_items && (!coded_bits || (sample_rates && !n_emit))) || (n_values && (!in_v || !out_v)) || limiter_ms < 0)
     return fail (ctx, "%s: bad arguments", name);
   if (snr_power)
@@ -2709,7 +2820,7 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
       covered += items[i].n_frames * uint64_t (items[i].channels);
       if (items[i].n_frames && !resampled (i))
         blist.push_back (batch_entry ((long long) items[i].value_offset, (long long) items[i].n_frames, items[i].channels, int (i), limiter_block44,
-                                      n_tiles44, n_lim44, n_peaks, zero_frames ? (long long) zero_frames[i] : 0));
+                                      n_tiles44, n_lim44, n_peaks, zero_frames ? (long long) zero_frames[i] : 0, role_table (i)));
     }
   const size_t n_list44 = blist.size();
   const size_t cap = scratch_bytes ? scratch_bytes : kBatchDefaultScratch;
@@ -2779,7 +2890,7 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
       if (R.limiter_block > 0)
         w.n_lim += (R.n_frames + 256 * kLimiterIter - 1) / (256 * kLimiterIter);
       /* WatermarkGen::run on every 1024-frame of the scratch copy (src/wmadd.cc:394-399): n_frames = n44, no limiter, no --snr */
-      blist.push_back (batch_entry ((long long) w.values, R.n44, R.C, int (i), 0, w.n_tiles, unused, unused, R.w0));
+      blist.push_back (batch_entry ((long long) w.values, R.n44, R.C, int (i), 0, w.n_tiles, unused, unused, R.w0, role_table (i)));
       soff.push_back (w.values);
       w.values += values;
       rlist.push_back (R);
@@ -2807,7 +2918,7 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
           CK (ctx->rate_items.reserve (rlist.size() * sizeof (RateItem)));
           CK (cudaMemcpyAsync (ctx->rate_items.p, rlist.data(), rlist.size() * sizeof (RateItem), cudaMemcpyHostToDevice, ctx->stream));
         }
-      const size_t coded_bytes = n_items * 2 * size_t (ctx->roles_n_coded);
+      const size_t coded_bytes = n_items * 2 * size_t (rs.n_coded);
       CK (ctx->batch_items.reserve (blist.size() * sizeof (BatchItem)));
       CK (ctx->batch_coded.reserve (coded_bytes));
       CK (cudaMemcpyAsync (ctx->batch_items.p, blist.data(), blist.size() * sizeof (BatchItem), cudaMemcpyHostToDevice, ctx->stream));
@@ -2824,7 +2935,7 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
         }
       double *d_snr = snr_power ? ctx->snr.as<double>() : nullptr;
       const BatchItem *d_b = ctx->batch_items.as<BatchItem>();
-      if (n_list44 && launch_embed_batch (ctx, d_in, d_out, d_b, int (n_list44), n_tiles44, n_lim44, frames_pad_start, water_delta, limiter_block44,
+      if (n_list44 && launch_embed_batch (ctx, rs, d_in, d_out, d_b, int (n_list44), n_tiles44, n_lim44, frames_pad_start, water_delta, limiter_block44,
                                           limiter_ceiling, d_snr, 0, zero_frames != nullptr))
         return 1;
       for (const Wave& w : waves)
@@ -2837,7 +2948,7 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
           PROF (ctx);
           (offsets ? k_resample_batch<true> : k_resample_batch<false>)<<<unsigned (w.n_rs), kRateCta, 0, ctx->stream>>> (d_r, n_r);
           LAUNCH_CHECK ("k_resample_batch");
-          if (launch_embed_batch (ctx, x44, x44 + w.values, d_b + w.b0, n_r, w.n_tiles, 0, frames_pad_start, water_delta, 0, limiter_ceiling, nullptr, 1,
+          if (launch_embed_batch (ctx, rs, x44, x44 + w.values, d_b + w.b0, n_r, w.n_tiles, 0, frames_pad_start, water_delta, 0, limiter_ceiling, nullptr, 1,
                                   offsets))
             return 1;
           PROF (ctx);
@@ -2909,6 +3020,24 @@ awm_embed_batch_rates_offsets (awm_ctx *ctx, const void *in_v, void *out_v, int 
   return embed_batch ("awm_embed_batch_rates_offsets", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, zero_frames, sample_rates,
                       n_emit, mark_sample_rate, frames_pad_start, water_delta, int ((long long) mark_sample_rate * limiter_ms / 1000), limiter_ms,
                       limiter_ceiling, snr_power, scratch_bytes);
+}
+
+int
+awm_embed_batch_keys (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                      const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, const uint64_t *zero_frames, const uint32_t *key_index,
+                      int mark_sample_rate, int frames_pad_start, double water_delta, int limiter_ms, float limiter_ceiling, double *snr_power,
+                      size_t scratch_bytes)
+{
+  if (!ctx->key_roles_n)
+    return fail (ctx, "awm_embed_batch_keys: awm_set_embed_roles_keys has not been called");
+  if (mark_sample_rate <= 0)
+    return fail (ctx, "awm_embed_batch_keys: mark sample rate %d must be > 0", mark_sample_rate);
+  char why[240];
+  if (awm_batch_keys_validate (items, n_items, n_values, sample_rates, n_emit, zero_frames, key_index, ctx->key_roles_n, mark_sample_rate, why, sizeof (why)))
+    return fail (ctx, "awm_embed_batch_keys: %s", why);
+  return embed_batch ("awm_embed_batch_keys", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, zero_frames, sample_rates, n_emit,
+                      mark_sample_rate, frames_pad_start, water_delta, int ((long long) mark_sample_rate * limiter_ms / 1000), limiter_ms, limiter_ceiling,
+                      snr_power, scratch_bytes, key_index);
 }
 
 /* ---------------------------------------------------------------- speed scan */

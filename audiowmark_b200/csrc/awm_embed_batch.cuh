@@ -1,5 +1,5 @@
-// awm_embed_batch.cuh -- batched embed: many items of one packed buffer, one key, one payload per item, in one launch of
-// k_embed_batch and one of k_limiter_batch (awm_embed_batch / awm_embed_batch_offsets in awm_capi.cu).
+// awm_embed_batch.cuh -- batched embed: many items of one packed buffer, one payload per item (and with awm_embed_batch_keys one key
+// per item), in one launch of k_embed_batch and one of k_limiter_batch (awm_embed_batch / awm_embed_batch_offsets in awm_capi.cu).
 //
 // Work list: every item with at least one sample-frame contributes ceil((F+1)/14) tiles of k_embed's shape (14 output frames +
 // one halo frame on each side) and ceil(F/4096) limiter CTAs; a CTA finds its item by binary search over the items' first tile
@@ -30,6 +30,7 @@ struct BatchItem
   long long frame0;            // stream 1024-frame where the processed range starts (0 for z < 2048)
   long long lead;              // processed positions before the item's first sample: z - 1024 * frame0, in [0, 2048)
   long long blk0;              // limiter block of stream position 1024 * frame0: peaks[peak0] belongs to it
+  int role_table;              // the item's role table: roles [role_table] (0 with one key per batch; awm_embed_batch_keys: its key's)
 };
 
 constexpr int kBatchRow = 104;           // per-warp frame-mod row in shared memory (101 bins, padded)
@@ -54,7 +55,8 @@ batch_item_of (const BatchItem *__restrict__ items, int n_items, long long cta)
 // base: the fields all items share (tables, strength, limiter block, peaks / snr base pointers, frame_number0 of a stream start);
 // in / out point to the packed buffer.  A tile's frames count from the item's frame0, positions from frame0 * 1024.
 // OFFSETS = false: every item starts its stream (frame0 = lead = blk0 = 0), the code of that case alone (awm_embed_batch).
-template<bool OFFSETS> __global__ void __launch_bounds__ (kEmbedWarps * 32, 1)
+// KEYS = true: every item reads its own role table roles [role_table] (awm_embed_batch_keys); false: all read roles [0].
+template<bool OFFSETS, bool KEYS> __global__ void __launch_bounds__ (kEmbedWarps * 32, 1)
 k_embed_batch (EmbedArgs base, const BatchItem *__restrict__ items, int n_items, const uint16_t *__restrict__ roles,
                const uint8_t *__restrict__ coded, int n_coded)
 {
@@ -85,7 +87,7 @@ k_embed_batch (EmbedArgs base, const BatchItem *__restrict__ items, int n_items,
   auto fm_row = [&] (long long r)
     {
       const int ab = r >= A.fpb;                            // rows [0,fpb) = A, [fpb,2fpb) = B
-      const uint16_t *role = roles + (size_t) (r - (long long) ab * A.fpb) * (kMaxBand + 1);
+      const uint16_t *role = roles + (size_t) (r + (long long) ((KEYS ? it.role_table : 0) - ab) * A.fpb) * (kMaxBand + 1);
       for (int k = lane; k <= kMaxBand; k += 32)
         row[k] = role_frame_mod (role[k], ab, item_coded + ab * n_coded);
       __syncwarp();

@@ -10,6 +10,7 @@
 
 #include <math.h>
 #include <functional>
+#include <map>
 
 using std::string;
 using std::vector;
@@ -276,6 +277,104 @@ add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, 
     : awm_embed_batch_rates (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), Params::mark_sample_rate,
                              Params::frames_pad_start, Params::water_delta, limiter_ms, Params::limiter_ceiling, snr, scratch_bytes);
   if (rc)
+    {
+      error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
+      return 1;
+    }
+  if (stats)
+    {
+      stats->resize (n_items);
+      for (size_t i = 0; i < n_items; i++)
+        (*stats)[i] = add_stats (runs[i], snr_power[2 * i], snr_power[2 * i + 1]);
+    }
+  return 0;
+}
+
+int
+add_watermark_batch_keys (const vector<Key>& keys, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                          const vector<string>& bits, const int *sample_rates, size_t scratch_bytes, vector<AddStats> *stats, const uint64_t *zero_frames)
+{
+  if (keys.size() != n_items || bits.size() != n_items)
+    {
+      error ("audiowmark: %zu items but %zu keys and %zu payloads\n", n_items, keys.size(), bits.size());
+      return 2;
+    }
+  /* the distinct keys in order of first use; item i uses key_index[i] of them */
+  vector<uint32_t> key_index (n_items);
+  vector<vector<unsigned char>> distinct;
+  std::map<vector<unsigned char>, uint32_t> seen;
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const vector<unsigned char> kb (keys[i].aes_key(), keys[i].aes_key() + Key::SIZE);
+      auto it = seen.find (kb);
+      if (it == seen.end())
+        {
+          it = seen.emplace (kb, uint32_t (distinct.size())).first;
+          distinct.push_back (kb);
+        }
+      key_index[i] = it->second;
+    }
+  char why[256];
+  if (awm_batch_keys_validate (items, n_items, n_values, sample_rates, nullptr, zero_frames, key_index.data(), distinct.size(), Params::mark_sample_rate,
+                               why, sizeof (why)))
+    {
+      error ("audiowmark: %s\n", why);
+      return 2;
+    }
+  /* every payload encoded with its own key's bit order, computed once per distinct key */
+  const size_t n_coded = code_size (ConvBlockType::a, Params::payload_size);
+  vector<vector<unsigned>> orders;
+  for (const auto& kb : distinct)
+    {
+      Key k;
+      k.set_key (kb.data(), "");
+      orders.push_back (bit_order (k, n_coded));
+    }
+  vector<uint8_t> coded;
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const vector<int> bitvec = parse_payload (bits[i]);
+      if (bitvec.empty())
+        return 2;
+      const vector<uint8_t> c = gen_coded_bits (orders[key_index[i]], bitvec);
+      coded.insert (coded.end(), c.begin(), c.end());
+    }
+  /* per item what the single-key call computes: frames through the mixer (other rates) and WatermarkGen::run calls */
+  vector<uint64_t> n_emit (n_items);
+  vector<size_t> runs (n_items);
+  for (size_t i = 0; i < n_items; i++)
+    {
+      const int rate = sample_rates ? sample_rates[i] : Params::mark_sample_rate;
+      const size_t block = size_t (rate) * size_t (Params::limiter_block_size_ms) / 1000;
+      const size_t z = zero_frames ? zero_frames[i] : 0, n_stream = z + items[i].n_frames;
+      if (rate == Params::mark_sample_rate)
+        {
+          runs[i] = gen_runs (n_stream, !Params::test_no_limiter, block);
+          continue;
+        }
+      size_t emit = 0;
+      resampled_add_plan (n_stream, rate, !Params::test_no_limiter, block, emit, runs[i]);
+      n_emit[i] = std::max<uint64_t> (emit, n_stream) - z;
+    }
+  awm_ctx *ctx = Engine::ctx();
+  if (!ctx)
+    return 1;
+  /* a call without items still needs a role set: that of the zero key, which no item reads */
+  vector<unsigned char> keys16 (std::max<size_t> (distinct.size(), 1) * Key::SIZE, 0);
+  for (size_t k = 0; k < distinct.size(); k++)
+    std::copy (distinct[k].begin(), distinct[k].end(), keys16.begin() + k * Key::SIZE);
+  const awm_role_layout layout = embed_role_layout();
+  if (awm_set_embed_roles_keys (ctx, keys16.data(), keys16.size() / Key::SIZE, &layout))
+    {
+      error ("audiowmark: %s\n", awm_last_error (ctx));
+      return 1;
+    }
+  vector<double> snr_power (2 * n_items);
+  const int limiter_ms = Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms);
+  double *snr = (Params::snr || stats) ? snr_power.data() : nullptr;
+  if (awm_embed_batch_keys (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, sample_rates ? n_emit.data() : nullptr,
+                            zero_frames, key_index.data(), Params::mark_sample_rate, Params::frames_pad_start, Params::water_delta, limiter_ms,
+                            Params::limiter_ceiling, snr, scratch_bytes))
     {
       error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
       return 1;

@@ -370,6 +370,79 @@ awmh_add_batch_rates_offsets_s16 (const unsigned char *key16, const int16_t *in,
                               zero_frames);
 }
 
+/* add_watermark_batch_keys on a packed buffer: keys16 [n_items][16] holds item i's key; zero_frames and sample_rates may be NULL
+ * (every item starts its stream / is at 44.1 kHz); otherwise as awmh_add_batch_rates_offsets.  Returns 2 on malformed input. */
+static int
+add_batch_keys_any (const unsigned char *keys16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                    const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks,
+                    double *snr_db)
+{
+  if (n_items && (!keys16 || !payload_hex))
+    return 2;
+  std::vector<Key> keys (n_items);
+  std::vector<std::string> bits (n_items);
+  for (size_t i = 0; i < n_items; i++)
+    {
+      keys[i] = make_key (keys16 + i * Key::SIZE, "");
+      bits[i] = payload_hex[i] ? payload_hex[i] : "";
+    }
+  std::vector<AddStats> stats;
+  const int rc = add_watermark_batch_keys (keys, in, out, s16, n_values, items, n_items, bits, sample_rates, scratch_bytes,
+                                           (data_blocks || snr_db) ? &stats : nullptr, zero_frames);
+  for (size_t i = 0; i < stats.size(); i++)
+    {
+      if (data_blocks)
+        data_blocks[i] = stats[i].data_blocks;
+      if (snr_db)
+        snr_db[i] = stats[i].snr_db;
+    }
+  return rc;
+}
+
+int
+awmh_add_batch_keys (const unsigned char *keys16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                     const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks,
+                     double *snr_db)
+{
+  return add_batch_keys_any (keys16, in, out, false, n_values, items, n_items, zero_frames, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
+}
+
+int
+awmh_add_batch_keys_s16 (const unsigned char *keys16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
+                         const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks,
+                         double *snr_db)
+{
+  return add_batch_keys_any (keys16, in, out, true, n_values, items, n_items, zero_frames, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
+}
+
+/* the role layout of the current Params (what awm_set_embed_roles_keys takes) as 6 ints in awm_role_layout's field order */
+void
+awmh_role_layout (int *out)
+{
+  const awm_role_layout l = embed_role_layout();
+  const int v[6] = { l.sync_frames, l.sync_frames_per_bit, l.data_frames, l.frames_per_bit, l.mix, l.n_coded_bits };
+  memcpy (out, v, sizeof (v));
+}
+
+/* role tables [n_keys][frames_per_block][101] of keys16 [n_keys][16] built on the device under the current Params (the tables
+ * awmh_embed_roles builds on the host one key at a time) */
+int
+awmh_embed_roles_device (const unsigned char *keys16, size_t n_keys, uint16_t *out, size_t out_size)
+{
+  awm_ctx *ctx = Engine::ctx();
+  if (!ctx)
+    return 1;
+  const awm_role_layout l = embed_role_layout();
+  if (n_keys * frames_per_block() * (Params::max_band + 1) > out_size)
+    return 2;
+  if (awm_set_embed_roles_keys (ctx, keys16, n_keys, &l) || awm_get_embed_roles_keys (ctx, 0, n_keys, out))
+    {
+      error ("audiowmark: %s\n", awm_last_error (ctx));
+      return 1;
+    }
+  return 0;
+}
+
 /* add / get between 16 bit PCM host buffers (the contents of a 16 bit WAV file): conversions run on the device */
 int
 awmh_add_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_frames, int n_channels, int sample_rate,

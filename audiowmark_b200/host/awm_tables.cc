@@ -190,6 +190,33 @@ gen_coded_bits (const Key& key, const std::vector<int>& bitvec)
 }
 
 std::vector<uint8_t>
+gen_coded_bits (const std::vector<unsigned>& order, const std::vector<int>& bitvec)
+{
+  std::vector<uint8_t> out;
+  for (ConvBlockType t : { ConvBlockType::a, ConvBlockType::b })
+    {
+      const std::vector<int> coded = code_encode (t, bitvec);
+      assert (coded.size() == order.size());
+      for (size_t i = 0; i < coded.size(); i++)
+        out.push_back (coded[order[i]]);                  // randomize_bit_order (encode)
+    }
+  return out;
+}
+
+awm_role_layout
+embed_role_layout()
+{
+  awm_role_layout l;
+  l.sync_frames = int (mark_sync_frame_count());
+  l.sync_frames_per_bit = Params::sync_frames_per_bit;
+  l.data_frames = int (mark_data_frame_count());
+  l.frames_per_bit = Params::frames_per_bit;
+  l.mix = Params::mix ? 1 : 0;
+  l.n_coded_bits = int (code_size (ConvBlockType::a, Params::payload_size));
+  return l;
+}
+
+std::vector<uint8_t>
 gen_frame_mod_ab (const Key& key, const std::vector<int>& bitvec)
 {
   const size_t fpb = frames_per_block(), n_bins = Params::max_band + 1;

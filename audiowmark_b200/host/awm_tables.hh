@@ -60,6 +60,10 @@ SyncTable gen_sync_table (const Key& key, int mode /* AWM_MODE_* */);
 std::vector<uint16_t> gen_embed_roles (const Key& key);
 /* coded data bits [2 (A, B)][n_coded] of one payload: randomize_bit_order (code_encode (A | B, bitvec)) */
 std::vector<uint8_t> gen_coded_bits (const Key& key, const std::vector<int>& bitvec);
+/* the same with the key's permutation given: order = bit_order (key, n_coded) */
+std::vector<uint8_t> gen_coded_bits (const std::vector<unsigned>& order, const std::vector<int>& bitvec);
+/* what gen_embed_roles depends on besides the key, under the current Params (awm_set_embed_roles_keys) */
+awm_role_layout embed_role_layout();
 /* FrameMod table [2][frames_per_block][101] for awm_set_embed_tables: 0 keep, 1 up, 2 down; roles x coded bits (empty on error) */
 std::vector<uint8_t> gen_frame_mod_ab (const Key& key, const std::vector<int>& bitvec);
 

@@ -37,6 +37,15 @@ int add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s
                                const std::vector<std::string>& bits, const int *sample_rates, size_t scratch_bytes, std::vector<AddStats> *stats,
                                const uint64_t *zero_frames = nullptr);
 
+/* add_watermark_batch_rates with a key per item (keys[i] for item i, keys.size() == n_items): item i comes out bit identical to the
+ * single-key batch call with keys[i], its stats as that call reports them.  sample_rates NULL: every item is at 44.1 kHz;
+ * zero_frames (optional) as in add_watermark_batch_rates.  The role tables of the distinct keys are built on the device once per call
+ * (awm_set_embed_roles_keys), each payload is encoded with its own key's bit order.  Returns 2 for a malformed item list, key list,
+ * rate, offset list or payload, 1 for other errors. */
+int add_watermark_batch_keys (const std::vector<Key>& keys, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items,
+                              size_t n_items, const std::vector<std::string>& bits, const int *sample_rates, size_t scratch_bytes,
+                              std::vector<AddStats> *stats, const uint64_t *zero_frames = nullptr);
+
 /* add_stream_watermark's loop with bounded memory (window by window; see awm_add.cc); callbacks read / write interleaved frames */
 int add_watermark_windowed (const Key& key, const std::function<Error (std::vector<float>&, size_t)>& read,
                             const std::function<Error (const std::vector<float>&)>& write, int n_channels, int sample_rate, const std::string& bits,

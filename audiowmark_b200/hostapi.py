@@ -18,7 +18,8 @@ CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
            "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_add_windowed",
            "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16", "awmh_add_batch_rates", "awmh_add_batch_rates_s16",
-           "awmh_add_batch_offsets", "awmh_add_batch_offsets_s16", "awmh_add_batch_rates_offsets", "awmh_add_batch_rates_offsets_s16"]
+           "awmh_add_batch_offsets", "awmh_add_batch_offsets_s16", "awmh_add_batch_rates_offsets", "awmh_add_batch_rates_offsets_s16",
+           "awmh_add_batch_keys", "awmh_add_batch_keys_s16", "awmh_role_layout", "awmh_embed_roles_device"]
 
 _lib = None
 
@@ -131,6 +132,49 @@ def embed_roles(key) -> np.ndarray:
     return out
 
 
+def role_layout() -> np.ndarray:
+    """awm_role_layout of the current parameters as int32 [6]: sync frames, sync frames per bit, data frames, frames per bit, mix,
+    coded bits"""
+    out = np.zeros(6, np.int32)
+    load().awmh_role_layout(_ptr(out))
+    return out
+
+
+def embed_roles_device(keys) -> np.ndarray:
+    """the role tables of many keys, built on the device in one launch: uint16 [len(keys), frames_per_block, 101], each equal to
+    embed_roles(key)"""
+    kb = _keys(keys, "embed_roles_device")
+    out = np.zeros((len(kb) // 16, frames_per_block(), 101), np.uint16)
+    if not out.size:
+        return out
+    rc = load().awmh_embed_roles_device(kb, ctypes.c_size_t(len(kb) // 16), _ptr(out), ctypes.c_size_t(out.size))
+    if rc:
+        raise RuntimeError("awmh_embed_roles_device failed (rc=%d); see stderr" % rc)
+    return out
+
+
+def _keys(keys, name, n=None) -> bytes:
+    """a list of 16-byte keys -> their concatenation (ValueError for a wrong key length or, with n, a wrong count)"""
+    keys = list(keys)
+    if n is not None and len(keys) != n:
+        raise ValueError("%s: %d items but %d keys" % (name, n, len(keys)))
+    kb = [bytes(k) for k in keys]
+    if any(len(k) != 16 for k in kb):
+        raise ValueError("%s: every key must be 16 bytes" % name)
+    return b"".join(kb)
+
+
+def _add_batch_keys(name, keys, key, s16, it, n_values, p_in, p_out, z, payloads, rates, scratch_bytes, stats):
+    """awmh_add_batch_keys[_s16] for add_batch / add_batch_rates with keys=; rates None: every item at 44.1 kHz"""
+    if key is not None:
+        raise ValueError("%s: pass either key= or keys=, not both" % name)
+    kb = _keys(keys, name, len(it))
+    pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
+    fn = load().awmh_add_batch_keys_s16 if s16 else load().awmh_add_batch_keys
+    return fn(kb if kb else None, p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), _ptr(z), pay, _ptr(rates),
+              ctypes.c_size_t(scratch_bytes), *stats)
+
+
 def coded_bits(key, payload_hex: str) -> np.ndarray:
     """one payload's coded data bits uint8 [2 (A, B), n_coded]: randomize_bit_order (code_encode (A | B, payload))"""
     out = np.zeros((2, n_coded_bits()), np.uint8)
@@ -229,7 +273,7 @@ def _zero_frames(name, zero_frames, n_items):
     return np.array([int(v) for v in z], np.uint64)
 
 
-def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False, zero_frames=None):
+def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False, zero_frames=None, keys=None):
     """`add` for many items with one key and one payload each, in one pass over the GPU; item i comes out bit identical to
     add / add_s16 of that item alone with payloads[i].
       pcms: a list of numpy arrays [n, channels] (all float32 or all int16; channels may differ), or one packed device tensor
@@ -239,6 +283,8 @@ def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None,
             frames earlier with silence, as an HLS segment does (`audiowmark hls-add`).  It comes out bit identical to
             add_windowed(item, payloads[i], zero_frames=zero_frames[i]) = add(zeros(z) ++ item)[z:] (16 bit: add_s16 of the same),
             with that call's data blocks and SNR.  zero_frames + n_frames is limited to 2^48 per item.
+      keys: None, or one 16-byte key per item (instead of key=): item i comes out bit identical to this call with key=keys[i].  The
+            role tables of the distinct keys are built on the device in one launch.
     Returns the list of outputs (numpy arrays, or views of the output tensor), with want_stats also the lists of data blocks
     and SNR dB per item.  Only 44.1 kHz input is accepted.  Raises ValueError for a malformed item list, offset list or payload."""
     payloads = list(payloads)
@@ -248,7 +294,11 @@ def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None,
     blocks = np.zeros(max(len(it), 1), np.int32)
     snr = np.zeros(max(len(it), 1), np.float64)
     stats = (_ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
-    if z is None:
+    if keys is not None:
+        if sample_rate != 44100:
+            raise ValueError("add_batch: only 44.1 kHz input is accepted (use add_batch_rates)")
+        rc = _add_batch_keys("add_batch", keys, key, s16, it, n_values, p_in, p_out, z, payloads, None, 0, stats)
+    elif z is None:
         fn = load().awmh_add_batch_s16 if s16 else load().awmh_add_batch
         rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, ctypes.c_int(sample_rate), *stats)
     else:
@@ -264,7 +314,7 @@ def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None,
     return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs
 
 
-def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None, want_stats=False, scratch_bytes=0, zero_frames=None):
+def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None, want_stats=False, scratch_bytes=0, zero_frames=None, keys=None):
     """add_batch for items that each have their own sample rate: item i comes out bit identical to add(item, payloads[i],
     sample_rate=sample_rates[i]) of that item alone (16 bit items: to that `add` between int16_to_float and 16 bit quantisation, what
     `audiowmark add` computes on a 16 bit file).  pcms / items / out / want_stats as in add_batch.  scratch_bytes: device scratch
@@ -273,6 +323,7 @@ def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None
     zero_frames[i] frames earlier with silence (an HLS segment of a 48 kHz master).  It comes out bit identical to
     add_batch_rates([zeros(z) ++ item], ...)[z:], with the data blocks of that whole stream and the SNR of the item's own positions;
     the silent prefix is never allocated.  zero_frames + n_frames is limited to 2^48 per item, at the item's rate and at 44.1 kHz.
+    keys: None, or one 16-byte key per item (instead of key=), as in add_batch.
     Raises ValueError for a malformed item list, rate list, offset list or payload."""
     payloads = list(payloads)
     rates = np.array([int(r) for r in sample_rates], np.int64)
@@ -287,7 +338,9 @@ def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None
     blocks = np.zeros(max(len(it), 1), np.int32)
     snr = np.zeros(max(len(it), 1), np.float64)
     stats = (_ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
-    if z is None:
+    if keys is not None:
+        rc = _add_batch_keys("add_batch_rates", keys, key, s16, it, n_values, p_in, p_out, z, payloads, rates, scratch_bytes, stats)
+    elif z is None:
         fn = load().awmh_add_batch_rates_s16 if s16 else load().awmh_add_batch_rates
         rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, _ptr(rates),
                 ctypes.c_size_t(scratch_bytes), *stats)

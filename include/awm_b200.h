@@ -243,6 +243,40 @@ int awm_embed_batch_rates_offsets (awm_ctx *ctx, const void *in, void *out, int 
                                    int mark_sample_rate, int frames_pad_start, double water_delta, int limiter_ms, float limiter_ceiling,
                                    double *snr_power, size_t scratch_bytes);
 
+/* ---- batched embed with a key per item ----------------------------------------------------------------------------------
+ * What the role table of a key (gen_embed_roles on the host: UpDownGen, BitPosGen and gen_mix_entries, src/wmcommon.cc:143-202)
+ * depends on besides the key: the frame counts of one block, frames_per_bit, --linear and the code length. */
+typedef struct {
+  int sync_frames;             /* sync_bits * sync_frames_per_bit (510) */
+  int sync_frames_per_bit;     /* 85 */
+  int data_frames;             /* n_coded_bits * frames_per_bit */
+  int frames_per_bit;          /* --frames-per-bit */
+  int mix;                     /* 0: --linear */
+  int n_coded_bits;            /* coded data bits per block: code_size (A, payload_size) */
+} awm_role_layout;
+/* builds the role tables uint16 [n_keys][sync_frames + data_frames][101] of n_keys 16-byte AES keys (keys16: [n_keys][16], host or
+ * device) on the device, each byte identical to the host's gen_embed_roles under this layout, and makes them the context's role set
+ * (replacing the previous one; awm_set_embed_roles's table is not touched).  Fails, leaving no role set, if a key's table would assign
+ * a (frame, bin) entry twice, as the host's builder does. */
+int awm_set_embed_roles_keys (awm_ctx *ctx, const uint8_t *keys16, size_t n_keys, const awm_role_layout *layout);
+/* copies the role tables of keys first_key .. first_key + n_keys - 1 of the role set to out (host or device) */
+int awm_get_embed_roles_keys (awm_ctx *ctx, size_t first_key, size_t n_keys, uint16_t *out);
+/* 0 if the validator of the matching single-key call passes (sample_rates NULL: awm_batch_offsets_validate's checks at
+ * mark_sample_rate with zero_frames optional; else awm_batch_rates_validate, or awm_batch_rates_offsets_validate when zero_frames is
+ * not NULL), key_index is not NULL and n_keys > 0 (for n_items > 0) and every key_index[i] < n_keys; else nonzero with the reason in
+ * err.  Needs no device. */
+int awm_batch_keys_validate (const awm_batch_item *items, size_t n_items, size_t n_values, const int *sample_rates, const uint64_t *n_emit,
+                             const uint64_t *zero_frames, const uint32_t *key_index, size_t n_keys, int mark_sample_rate, char *err, size_t err_cap);
+/* awm_embed_batch_rates_offsets with a key per item: item i is embedded with role table key_index[i] of the role set
+ * (awm_set_embed_roles_keys) and its coded bits coded_bits[i] (randomize_bit_order with its own key), and comes out bit identical to
+ * the single-key call with that key.  sample_rates NULL: every item is at mark_sample_rate (n_emit is then ignored); zero_frames
+ * NULL: every item starts its stream.  coded_bits: uint8 [n_items][2][n_coded_bits of the role set].  Everything else as
+ * awm_embed_batch_rates_offsets. */
+int awm_embed_batch_keys (awm_ctx *ctx, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
+                          const uint8_t *coded_bits, const int *sample_rates, const uint64_t *n_emit, const uint64_t *zero_frames,
+                          const uint32_t *key_index, int mark_sample_rate, int frames_pad_start, double water_delta, int limiter_ms,
+                          float limiter_ceiling, double *snr_power, size_t scratch_bytes);
+
 /* ---- sync search on the bound PCM --------------------------------------------------------
  * awm_sync_approx = SyncFinder::search_approx (src/syncfinder.cc:171-256): for the four
  * 256-sample shifts the channel-summed dB spectrogram (sync_fft, :560-605), sync_decode (:116-153)
