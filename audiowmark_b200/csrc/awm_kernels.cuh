@@ -555,14 +555,15 @@ k_mix_decode (const float *__restrict__ D, int n_blk, int C, int frames_per_bloc
 
 // =============================================================================================
 // normalize_soft_bits (src/wmget.cc:40-65) + conv_decode_soft (src/convcode.cc:128-213).
-// One CTA = one code word; decision word u (32 consecutive new states 32u..32u+31) is computed by one thread.
+// One CTA = one code word; decision word u (32 consecutive new states 32u..32u+31) of a trellis step is computed by one thread.
 //   new_state ns has predecessors ps0 = ns>>1 and ps1 = ps0 + 2^14; the reference visits old
 //   states in ascending order and replaces only on strict '<', so ps1 wins only if strictly better.
 //   path metric: delta = (((old + m_0) + m_1) + ...) in float, m_p = (c_p - s_p)^2 as the reference.
 // =============================================================================================
 constexpr int kVitStates = 1 << AWM_VITERBI_ORDER;
-constexpr int kVitThreads = 512;      // CTA size; each thread owns two groups of 32 new states
 constexpr int kVitWords = kVitStates / 32;   // decision words per trellis step
+constexpr int kVitThreads = kVitWords;       // CTA size; thread i computes decision word i of a full trellis step
+constexpr int kVitLgWords = AWM_VITERBI_ORDER - 5;
 
 // generator polynomials (src/convcode.cc:42-46) as compile-time constants: A = even, B = odd, AB = all
 __host__ __device__ constexpr unsigned ab_generator (int i)
@@ -573,100 +574,177 @@ __host__ __device__ constexpr unsigned ab_generator (int i)
 template<int TYPE> __host__ __device__ constexpr unsigned type_generator (int p) { return TYPE == AWM_BLOCK_AB ? ab_generator (p) : ab_generator (2 * p + TYPE); }
 __host__ __device__ constexpr bool cparity (unsigned v) { v ^= v >> 16; v ^= v >> 8; v ^= v >> 4; v ^= v >> 2; v ^= v >> 1; return v & 1u; }
 
-// One trellis step for the 32 new states ns = 32u + q of group u; returns the 32 decision bits.
-// The output bit p of state ns is parity (ns & g_p) = parity (32u & g_p) ^ parity (q & g_p): the first factor
-// is a per-group constant (hi, bit p), the second a compile-time constant, so which of (c-0)^2 / (c-1)^2 is
-// added needs no instruction at all inside the unrolled loops.
-// shared-memory position of path metric n: four floats of padding after every 32, so that the float4 accesses of a quarter warp
-// (reads 64 bytes apart, writes 128 bytes apart in the unpadded array) fall into eight different bank groups
-__device__ __forceinline__ int vit_pos (int n) { return n + ((n >> 5) << 2); }
-constexpr int kVitPadded = kVitStates + kVitStates / 32 * 4;
+/* In-place path metrics.  New states 2j and 2j+1 have the same two predecessors j and j + 2^14, so one thread reads those two
+ * metrics and writes the two new ones over them: new state 2j takes the place of j, 2j+1 that of j + 2^14.  The position of
+ * state x after t steps is therefore x rotated right by t within 15 bits; vit_rot applies the rotation, vit_fold then XORs the
+ * three 5-bit digits of the position into the lowest one (the shared-memory bank).  Both maps are linear over GF(2), so a
+ * position is the XOR of the positions of the state's bits, and five consecutive state bits always land on five different bank
+ * bits: the 32 lanes of a warp, which differ in five consecutive bits of the word index, hit 32 different banks at every step. */
+__device__ __forceinline__ unsigned vit_rot (unsigned x, int r) { return ((x >> r) | (x << (AWM_VITERBI_ORDER - r))) & (kVitStates - 1); }
+__device__ __forceinline__ unsigned vit_fold (unsigned a) { return a ^ (((a >> 5) ^ (a >> 10)) & 31u); }
+__device__ __forceinline__ unsigned vit_pos (unsigned x, int r) { return vit_fold (vit_rot (x, r)); }
 
-// d_lo / d_hi: the path metrics of the predecessors ps0 = 16 u + .. (lower half of the states) and ps1 = ps0 + 2^14 (upper half),
-// both addressed with vit_pos (16 u + ..)
-template<int TYPE> __device__ __forceinline__ uint32_t
-viterbi_step (const float *__restrict__ d_lo, const float *__restrict__ d_hi, float (&outv)[32], unsigned hi, const float *m0, const float *m1, int u)
+// One trellis step for the 32 new states ns = 32u + k of word u; returns the 32 decision bits.
+// The output bit p of state ns is parity (ns & g_p) = parity (32u & g_p) ^ parity (k & g_p): the first factor
+// is a per-word constant (hi, bit p), the second a compile-time constant, so which of (c-0)^2 / (c-1)^2 is
+// added needs no instruction at all inside the unrolled loops.
+// Positions are in bytes: pos of predecessor 16u, cq.x .. cq.w of predecessor bits 0 .. 3, ch of bit 14 (ps1 = ps0 ^ 2^14).
+// QS = 0 computes all 32 states; QS > 0 only the states k = 2q with q a multiple of QS: the positions of the others are not
+// written and their decision bits are 0.
+template<int TYPE, int QS> __device__ __forceinline__ uint32_t
+viterbi_word (float *dm, unsigned pos, uint4 cq, unsigned ch, unsigned hi, const float4 *m)
 {
   constexpr int RATE = TYPE == AWM_BLOCK_AB ? 12 : 6;
-  // The two candidates of a new state -- coming from predecessor ps0 and from ps1 -- add the SAME branch metrics in the same order,
-  // so they travel as one pair (d0, d1) through the f2 helpers (awm_f32x2.cuh), every half rounded exactly like __fadd_rn.
+  constexpr int QSTEP = QS ? QS : 1;
+  // The two candidates of a new state -- coming from predecessor ps0 and from ps1 -- add the SAME branch metrics in the same order;
+  // where both are summed they travel as one pair (d0, d1) through the f2 helpers (awm_f32x2.cuh), every half rounded exactly
+  // like __fadd_rn.
   f2 mA[RATE], mB[RATE];                  // (m, m): metric for output bit == hi-bit / != hi-bit
 #pragma unroll
   for (int p = 0; p < RATE; p++)
     {
-      const bool h = (hi >> p) & 1u;
-      const float a = h ? m1[p] : m0[p], b = h ? m0[p] : m1[p];
-      mA[p] = f2_make (a, a);
-      mB[p] = f2_make (b, b);
+      // m[p] = (m0, m1, m1, m0): the pair at float offset 2 * (hi bit p) is (metric for hi bit, metric for its complement)
+      const unsigned off = (p <= 3 ? hi << (3 - p) : hi >> (p - 3)) & 8u;
+      const float2 ab = *reinterpret_cast<const float2 *> (reinterpret_cast<const char *> (m + p) + off);
+      mA[p] = f2_make (ab.x, ab.x);
+      mB[p] = f2_make (ab.y, ab.y);
     }
+  char *base = reinterpret_cast<char *> (dm);
+  // byte position of predecessor 16u + q, and of its partner 16u + q + 2^14
+  const auto at = [&] (int q) { return pos ^ ((q & 1) ? cq.x : 0u) ^ ((q & 2) ? cq.y : 0u) ^ ((q & 4) ? cq.z : 0u) ^ ((q & 8) ? cq.w : 0u); };
+  const auto ptr = [&] (unsigned a) { return reinterpret_cast<float *> (base + a); };
   uint32_t word = 0;
+  float *p0 = ptr (at (16 - QSTEP)), *p1 = ptr (at (16 - QSTEP) ^ ch);
+  f2 d01 = f2_make (*p0, *p1);
 #pragma unroll
-  for (int v = 0; v < 4; v++)                                // 8 new states <- 4 + 4 predecessors
+  for (int q = 16 - QSTEP; q >= 0; q -= QSTEP)              // new states 2q, 2q+1 <- predecessors 16u + q, 16u + q + 2^14
     {
-      const float4 x = *reinterpret_cast<const float4 *> (d_lo + vit_pos (16 * u + 4 * v));
-      const float4 y = *reinterpret_cast<const float4 *> (d_hi + vit_pos (16 * u + 4 * v));
-      const f2 a01[4] = { f2_make (x.x, y.x), f2_make (x.y, y.y), f2_make (x.z, y.z), f2_make (x.w, y.w) };
-#pragma unroll
-      for (int q = 0; q < 8; q++)
+      // the next pair's metrics are loaded before this pair's are stored (different positions), so the load latency overlaps the adds
+      float *n0 = p0, *n1 = p1;
+      f2 next = d01;
+      if (q >= QSTEP)
         {
-          f2 d = a01[q >> 1];
+          n0 = ptr (at (q - QSTEP));
+          n1 = ptr (at (q - QSTEP) ^ ch);
+          next = f2_make (*n0, *n1);
+        }
+      /* The new metric of a state is min (F (x), F (y)), F (v) = ((v + m_0) + m_1) + ... in float, x / y the metrics of ps0 / ps1, and
+       * ps1 is taken iff F (y) < F (x).  Every rounded add is monotonic, so x <= y gives F (x) <= F (y): ps0, metric F (x).  y < x
+       * gives F (y) <= F (x), so the metric is F (y) either way, and ps1 is taken unless the rounding merges the two sums.  Each add
+       * brings them at most one ulp of its result closer, at most ulp (F (x)) <= 2^-23 F (x) + 2^-149; with RATE <= 12 adds and
+       * F (x) < (1 + 2^-19) (F (y) + (x - y)) + 2^-145 that stays short of x - y once x - y > 2^-18 F (y) + 2^-140 (a margin of 2.6 for the
+       * roundings of the test itself).  So one sum per state decides, and both sums are compared, as the reference does, only for
+       * the rare pairs closer than that -- and for NaN, where neither comparison holds. */
+      const float x = d01.x, y = d01.y;
+      const float h = __fsub_rn (y, x);                       // sign set iff y < x (never -0; inf - inf is a positive NaN)
+      const float mn = h < 0.f ? y : x;
+      float out[2], sg[2];
+#pragma unroll
+      for (int s = QS ? 0 : 1; s >= 0; s--)
+        {
+          float d = mn;
 #pragma unroll
           for (int p = 0; p < RATE; p++)
-            d = f2_add (d, cparity (unsigned (8 * v + q) & type_generator<TYPE> (p)) ? mB[p] : mA[p]);
-          float d0, d1;
-          f2_split (d, d0, d1);
-          const bool take1 = d1 < d0;
-          outv[8 * v + q] = take1 ? d1 : d0;
-          word |= (take1 ? 1u : 0u) << (8 * v + q);
+            d = __fadd_rn (d, cparity (unsigned (2 * q + s) & type_generator<TYPE> (p)) ? mB[p].x : mA[p].x);
+          out[s] = d;
+          sg[s] = h;
         }
+      const float top = QS ? out[0] : fmaxf (out[0], out[1]);
+      if (!(x <= y || -h > __fmaf_rn (top, 0x1p-18f, 0x1p-140f)))
+        {
+#pragma unroll
+          for (int s = QS ? 0 : 1; s >= 0; s--)
+            {
+              f2 d = d01;
+#pragma unroll
+              for (int p = 0; p < RATE; p++)
+                d = f2_add (d, cparity (unsigned (2 * q + s) & type_generator<TYPE> (p)) ? mB[p] : mA[p]);
+              float d0, d1;
+              f2_split (d, d0, d1);
+              /* take ps1 iff d1 < d0: exactly when d1 - d0 is negative (the difference of two different floats never rounds to
+               * 0, inf - inf is a positive NaN), and then min (d0, d1) is d1.  Metrics are never -0, and NaN in one candidate
+               * means NaN in both (digital silence aside, which never gets here). */
+              sg[s] = __fsub_rn (d1, d0);
+              out[s] = fminf (d0, d1);
+            }
+        }
+#pragma unroll
+      for (int s = QS ? 0 : 1; s >= 0; s--)
+        if constexpr (QS == 0)
+          word = __funnelshift_l (__float_as_uint (sg[s]), word, 1);    // the sign bits enter the word from the low end
+        else
+          word |= (__float_as_uint (sg[s]) >> 31) << (2 * q);
+      *p0 = out[0];
+      if constexpr (QS == 0)
+        *p1 = out[1];
+      p0 = n0;
+      p1 = n1;
+      d01 = next;
     }
   return word;
 }
 
-// The 2^15 path metrics of a code word live in shared memory (128 KB).  A trellis step reads the two predecessors of every new
-// state, so the update cannot be done in place state by state; instead every thread keeps the 64 new metrics of its two groups in
-// registers until the whole CTA has read the old ones (barrier), then stores them over the old array (barrier).  No metric ever
-// travels to L2 / HBM; only the decision bits (4 KB per step, read back once by the traceback) are written to global memory.
+// The 2^15 path metrics of a code word live in shared memory (128 KB) and are updated in place, one barrier per step.  No metric
+// ever travels to L2 / HBM; only the decision bits (4 KB per step, read back once by the traceback) are written to global memory.
+// Words that cannot matter are skipped:
+//   - the trellis starts in state 0, so after step t only new states < 2^(t+1) are reachable: the other metrics stay +inf (their
+//     positions are never written, and the rotation maps unreachable states onto unreachable states);
+//   - the traceback starts in state 0, so with r steps left after step t only new states that are multiples of 2^(15-r) are on a
+//     path that ends there; the others are neither read by those states nor visited by the traceback.
+// Step t computes the words u = i * 2^lg_m, i < 2^(lg_f - lg_m): the multiples of the second stride among the first 2^lg_f words,
+// and in the last 15 steps only the states of those words that are multiples of the second stride.
 template<int TYPE> __device__ __forceinline__ void
-viterbi_run (float *dm, uint32_t *dec, const float *coded, float *m0, float *m1, int steps, int tid)
+viterbi_run (float *dm, uint32_t *dec, const float *coded, float4 *m, const uint4 *rq, const unsigned *rh, int steps, int tid)
 {
   constexpr int RATE = TYPE == AWM_BLOCK_AB ? 12 : 6;
-  constexpr int kGroups = kVitWords / kVitThreads;
-  unsigned hi[kGroups];
-#pragma unroll
-  for (int g = 0; g < kGroups; g++)
+  unsigned cur_u = ~0u, hi = 0;
+  int rot = 0;                                              // t mod 15
+  if (tid < RATE)
     {
-      const unsigned base = 32u * unsigned (tid + g * kVitThreads);
-      hi[g] = 0;
-#pragma unroll
-      for (int p = 0; p < RATE; p++)
-        hi[g] |= unsigned (__popc (base & type_generator<TYPE> (p)) & 1) << p;
+      const float c = coded[tid];
+      const float m0 = __fmul_rn (c, c), m1 = __fmul_rn (c - 1.0f, c - 1.0f);   // (c - 0)^2, (c - 1)^2
+      m[tid] = make_float4 (m0, m1, m1, m0);
     }
   for (int t = 0; t < steps; t++)
     {
-      if (tid < RATE)
+      __syncthreads();                                      // metrics of the previous step stored, m[t & 1] ready
+      if (tid < RATE && t + 1 < steps)                      // branch metrics of the next step into the other buffer
         {
-          const float c = coded[t * RATE + tid];
-          m0[tid] = __fmul_rn (c, c);                       // (c - 0)^2
-          m1[tid] = __fmul_rn (c - 1.0f, c - 1.0f);         // (c - 1)^2
+          const float c = coded[(t + 1) * RATE + tid];
+          const float m0 = __fmul_rn (c, c), m1 = __fmul_rn (c - 1.0f, c - 1.0f);
+          m[((t + 1) & 1) * 12 + tid] = make_float4 (m0, m1, m1, m0);
         }
-      __syncthreads();                                      // metrics of the previous step stored, m0 / m1 ready
-      float outv[kGroups][32];
-#pragma unroll
-      for (int g = 0; g < kGroups; g++)
+      const int left = steps - 1 - t;
+      const int lg_f = min (kVitLgWords, max (0, t - 4));
+      const int lg_m = left >= kVitLgWords ? 0 : kVitLgWords - left;
+      const int n = lg_f > lg_m ? 1 << (lg_f - lg_m) : 1;
+      if (tid < n)
         {
-          const int u = tid + g * kVitThreads;
-          dec[(size_t) t * kVitWords + u] = viterbi_step<TYPE> (dm, dm + vit_pos (kVitStates >> 1), outv[g], hi[g], m0, m1, u);
-        }
-      __syncthreads();                                      // every thread has read its predecessors
+          const unsigned u = unsigned (tid) << lg_m;
+          if (u != cur_u)
+            {
+              cur_u = u;
+              hi = 0;
 #pragma unroll
-      for (int g = 0; g < kGroups; g++)
-        {
-          float4 *on = reinterpret_cast<float4 *> (dm + vit_pos (32 * (tid + g * kVitThreads)));
-#pragma unroll
-          for (int k = 0; k < 8; k++)
-            on[k] = make_float4 (outv[g][4 * k], outv[g][4 * k + 1], outv[g][4 * k + 2], outv[g][4 * k + 3]);
+              for (int p = 0; p < RATE; p++)
+                hi |= unsigned (__popc ((32u * u) & type_generator<TYPE> (p)) & 1) << p;
+            }
+          const unsigned pos = 4 * vit_pos (16u * u, rot), ch = rh[rot];
+          const uint4 cq = rq[rot];
+          const float4 *mt = m + (t & 1) * 12;
+          uint32_t word;
+          // with left < 15 the states used later are the multiples of 2^(15 - left): k = 2q in word u, q a multiple of 2^(14 - left)
+          switch (left)
+            {
+            case 14: word = viterbi_word<TYPE, 1> (dm, pos, cq, ch, hi, mt); break;
+            case 13: word = viterbi_word<TYPE, 2> (dm, pos, cq, ch, hi, mt); break;
+            case 12: word = viterbi_word<TYPE, 4> (dm, pos, cq, ch, hi, mt); break;
+            case 11: word = viterbi_word<TYPE, 8> (dm, pos, cq, ch, hi, mt); break;
+            default: word = left < 11 ? viterbi_word<TYPE, 16> (dm, pos, cq, ch, hi, mt) : viterbi_word<TYPE, 0> (dm, pos, cq, ch, hi, mt); break;
+            }
+          dec[(size_t) t * kVitWords + u] = word;
         }
+      rot = rot == AWM_VITERBI_ORDER - 1 ? 0 : rot + 1;
     }
   __syncthreads();
 }
@@ -710,17 +788,19 @@ viterbi_traceback (const uint32_t *dec, int steps, int n_msg, unsigned char *bit
     }
 }
 
-constexpr size_t viterbi_smem_bytes (int steps) { return size_t (kVitPadded) * sizeof (float) + size_t (steps) * 12 * sizeof (float); }
+constexpr size_t viterbi_smem_bytes (int steps) { return size_t (kVitStates) * sizeof (float) + size_t (steps) * 12 * sizeof (float); }
 
-__global__ void __launch_bounds__ (kVitThreads)
+__global__ void __launch_bounds__ (kVitThreads, 1)
 k_viterbi (const float *__restrict__ raw, const long long *__restrict__ raw_off, int n_msg, const int *__restrict__ block_types, int hard,
            int max_steps, uint32_t *__restrict__ dec_buf /* [job][steps][kVitWords] */,
            unsigned char *__restrict__ bits_out, float *__restrict__ err_out)
 {
   extern __shared__ __align__ (16) unsigned char smem[];
-  float *dm = reinterpret_cast<float *> (smem);             // [2^15] path metrics (padded, vit_pos)
-  float *coded = dm + kVitPadded;                           // [n_coded] normalised soft bits
-  __shared__ float m0[12], m1[12];
+  float *dm = reinterpret_cast<float *> (smem);             // [2^15] path metrics (in place, vit_pos)
+  float *coded = dm + kVitStates;                           // [n_coded] normalised soft bits
+  __shared__ float4 m[2][12];                               // branch metrics of two consecutive steps (viterbi_word)
+  __shared__ uint4 rq[AWM_VITERBI_ORDER];                   // byte positions of state bits 0 .. 3 at each rotation
+  __shared__ unsigned rh[AWM_VITERBI_ORDER];                // and of state bit 14
   __shared__ double s_mean;
   const int job = blockIdx.x, tid = threadIdx.x;
   const int btype = block_types[job];
@@ -728,41 +808,52 @@ k_viterbi (const float *__restrict__ raw, const long long *__restrict__ raw_off,
   const int steps = n_msg + AWM_VITERBI_ORDER;
   const int n_coded = steps * rate;
 
+  // the raw soft bits are staged in shared memory first: the mean below is one serial sum, whose loads then wait on shared memory
   const float *rj = raw + raw_off[job];
-  if (tid == 0)
+  for (int i = tid; i < n_coded; i += blockDim.x)
+    coded[i] = rj[i];
+  for (int i = tid; i < kVitStates; i += blockDim.x)
+    dm[i] = (i == 0) ? 0.f : INFINITY;                      // state 0 at position 0 whatever the rotation
+  if (tid < AWM_VITERBI_ORDER)
     {
-      double mean = 0;
-      for (int i = 0; i < n_coded; i++)
-        mean += fabs (double (rj[i]));
-      s_mean = mean / n_coded;
+      rq[tid] = make_uint4 (4 * vit_pos (1u, tid), 4 * vit_pos (2u, tid), 4 * vit_pos (4u, tid), 4 * vit_pos (8u, tid));
+      rh[tid] = 4 * vit_pos (unsigned (kVitStates >> 1), tid);
     }
   __syncthreads();
-  /* digital silence: every raw soft bit is exactly 0, so mean == 0 and normalize_soft_bits (src/wmget.cc:56-61) yields 0/0 = NaN for
-   * every coded bit (raw values are finite sums of dB values, so NaN is all-or-nothing).  In conv_decode_soft (src/convcode.cc:164-190)
-   * the NaN path metrics of step 0 fail the "old_table[state].delta >= 0" reachability test of step 1: every later table keeps its
-   * initial StateEntry {0, -1, 0}, the traceback reads bit 0 / last_state 0 everywhere and error_out = -1 / n_coded. */
-  if (!hard && !(s_mean > 0))
+  if (!hard)
     {
-      for (int i = tid; i < n_msg; i += blockDim.x)
-        bits_out[(size_t) job * n_msg + i] = 0;
       if (tid == 0)
-        err_out[job] = -1.0f / float (n_coded);
-      return;
+        {
+          double mean = 0;
+          for (int i = 0; i < n_coded; i++)
+            mean += fabs (double (coded[i]));
+          s_mean = mean / n_coded;
+        }
+      __syncthreads();
+      /* digital silence: every raw soft bit is exactly 0, so mean == 0 and normalize_soft_bits (src/wmget.cc:56-61) yields 0/0 = NaN for
+       * every coded bit (raw values are finite sums of dB values, so NaN is all-or-nothing).  In conv_decode_soft (src/convcode.cc:164-190)
+       * the NaN path metrics of step 0 fail the "old_table[state].delta >= 0" reachability test of step 1: every later table keeps its
+       * initial StateEntry {0, -1, 0}, the traceback reads bit 0 / last_state 0 everywhere and error_out = -1 / n_coded. */
+      if (!(s_mean > 0))
+        {
+          for (int i = tid; i < n_msg; i += blockDim.x)
+            bits_out[(size_t) job * n_msg + i] = 0;
+          if (tid == 0)
+            err_out[job] = -1.0f / float (n_coded);
+          return;
+        }
     }
   for (int i = tid; i < n_coded; i += blockDim.x)
-    coded[i] = hard ? (rj[i] > 0 ? 1.0f : 0.0f) : float (0.5 * (double (rj[i]) / s_mean + 1));
-
+    coded[i] = hard ? (coded[i] > 0 ? 1.0f : 0.0f) : float (0.5 * (double (coded[i]) / s_mean + 1));
   uint32_t *dec = dec_buf + (size_t) job * max_steps * kVitWords;
-  for (int i = tid; i < kVitStates; i += blockDim.x)
-    dm[vit_pos (i)] = (i == 0) ? 0.f : INFINITY;
   __syncthreads();
 
   if (btype == AWM_BLOCK_A)
-    viterbi_run<AWM_BLOCK_A> (dm, dec, coded, m0, m1, steps, tid);
+    viterbi_run<AWM_BLOCK_A> (dm, dec, coded, &m[0][0], rq, rh, steps, tid);
   else if (btype == AWM_BLOCK_B)
-    viterbi_run<AWM_BLOCK_B> (dm, dec, coded, m0, m1, steps, tid);
+    viterbi_run<AWM_BLOCK_B> (dm, dec, coded, &m[0][0], rq, rh, steps, tid);
   else
-    viterbi_run<AWM_BLOCK_AB> (dm, dec, coded, m0, m1, steps, tid);
+    viterbi_run<AWM_BLOCK_AB> (dm, dec, coded, &m[0][0], rq, rh, steps, tid);
   if (tid == 0)
     err_out[job] = dm[0] / float (n_coded);
   if (tid < 32)
