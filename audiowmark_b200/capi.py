@@ -29,7 +29,7 @@ EXPORTS = [
     "awm_create", "awm_destroy", "awm_last_error", "awm_launch_count", "awm_stream", "awm_synchronize",
     "awm_profile_enable", "awm_profile_report", "awm_host_alloc", "awm_host_free",
     "awm_fft_r2c", "awm_fft_c2r", "awm_set_embed_tables", "awm_set_sync_tables", "awm_set_mix_tables",
-    "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_approx_enqueue", "awm_sync_use_slot", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_sync_refine_rescored", "awm_decode_blocks", "awm_viterbi",
+    "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_approx_enqueue", "awm_sync_use_slot", "awm_sync_have", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_sync_refine_rescored", "awm_decode_blocks", "awm_viterbi",
     "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_is_device_pointer", "awm_speed_scan", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_prefetch_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
     "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch", "awm_batch_rates_validate", "awm_embed_batch_rates",
     "awm_batch_offsets_validate", "awm_embed_batch_offsets", "awm_batch_rates_offsets_validate", "awm_embed_batch_rates_offsets",
@@ -290,6 +290,28 @@ class Context:
         self._ck(self.lib.awm_sync_approx(self.h, ctypes.c_int(key_slot), ctypes.c_int(mode), ctypes.c_uint64(wav_first), ctypes.c_uint64(wav_last),
                                           ctypes.c_double(water_delta), None, ctypes.c_size_t(0), ctypes.byref(n)))
         return n.value
+
+    def sync_approx_enqueue(self, slot: int, key_slot=0, mode=MODE_BLOCK, wav_first=0, wav_last=None, water_delta=0.01):
+        """awm_sync_approx_enqueue: queue the search into approx slot `slot` (the bound PCM must be the caller's device memory)"""
+        if wav_last is None:
+            wav_last = 0xFFFFFFFFFFFFFFF
+        self._ck(self.lib.awm_sync_approx_enqueue(self.h, ctypes.c_int(slot), ctypes.c_int(key_slot), ctypes.c_int(mode), ctypes.c_uint64(wav_first),
+                                                  ctypes.c_uint64(wav_last), ctypes.c_double(water_delta)))
+
+    def sync_use_slot(self, slot: int) -> int:
+        """awm_sync_use_slot: make approx slot `slot` current; returns its number of scores"""
+        n = ctypes.c_size_t()
+        self._ck(self.lib.awm_sync_use_slot(self.h, ctypes.c_int(slot), ctypes.byref(n)))
+        return n.value
+
+    def sync_have(self) -> np.ndarray:
+        """awm_sync_have: [4][frame_count - 1] bool, the frames the current slot's last search analysed"""
+        n = ctypes.c_size_t()
+        self._ck(self.lib.awm_sync_have(self.h, None, ctypes.c_size_t(0), ctypes.byref(n)))
+        out = np.zeros((4, n.value), np.uint8)
+        if n.value:
+            self._ck(self.lib.awm_sync_have(self.h, _ptr(out), ctypes.c_size_t(out.size), ctypes.byref(n)))
+        return out.astype(bool)
 
     def sync_peaks(self, min_abs_quality: float, max_peaks: int = 65536):
         """local maxima above a floor of the LAST sync_approx call; returns (peaks sorted by index, number found)."""

@@ -122,6 +122,7 @@ struct SyncTab
   int n_chunks = 0;
   int n_groups = 0;
   int n_ent = 0, n_bits = 0, total_frames = 0;
+  int max_frame = 0;                  // largest entry frame: a search needs it inside the block (frames_per_block, twice that in CLIP mode)
   std::vector<awm_sync_entry> h_ent;
   std::vector<int> h_off;
 };
@@ -177,6 +178,7 @@ struct awm_ctx
   {
     DevBuf have, q, scores, a_ud, a_cnt;
     size_t n_scores = 0;
+    long long n_have = 0; int ld_have = 0;                                // have[4][ld_have]: frames per shift written by the search
     const float *pcm = nullptr; size_t pcm_frames = 0; int pcm_ch = 0;    // the PCM view the search ran on
     cudaEvent_t done = nullptr;                                           // recorded after k_local_mean
   };
@@ -696,12 +698,31 @@ awm_set_sync_tables (awm_ctx *ctx, int key_slot, int mode, const awm_sync_entry 
 {
   if (key_slot < 0 || key_slot >= AWM_MAX_KEYS || mode < 0 || mode > 1 || !entries || n_entries <= 0 || !bit_offsets || n_bits <= 0)
     return fail (ctx, "awm_set_sync_tables: bad arguments");
+  /* every check comes before the slot is touched: a rejected table leaves the previous one in place, whole */
+  if (n_bits > 6)
+    return fail (ctx, "awm_set_sync_tables: at most 6 sync bits are supported");
   if (bit_offsets[0] != 0 || bit_offsets[n_bits] != n_entries)
     return fail (ctx, "awm_set_sync_tables: bit_offsets must run from 0 to n_entries");
+  for (int b = 0; b < n_bits; b++)
+    if (bit_offsets[b + 1] < bit_offsets[b])
+      return fail (ctx, "awm_set_sync_tables: bit_offsets must not decrease (bit %d)", b);
+  int max_frame = 0;
   for (int i = 0; i < n_entries; i++)
-    for (int j = 0; j < kUD; j++)
-      if (entries[i].up[j] >= kBands || entries[i].down[j] >= kBands)
-        return fail (ctx, "awm_set_sync_tables: band index out of range");
+    {
+      /* the tensor-core kernel sums an entry's bands through a 0/1 mask, so a band can count only once per list */
+      uint32_t seen_up[3] = { 0, 0, 0 }, seen_down[3] = { 0, 0, 0 };
+      for (int j = 0; j < kUD; j++)
+        {
+          const int u = entries[i].up[j], d = entries[i].down[j];
+          if (u >= kBands || d >= kBands)
+            return fail (ctx, "awm_set_sync_tables: band index out of range");
+          if ((seen_up[u >> 5] >> (u & 31)) & 1 || (seen_down[d >> 5] >> (d & 31)) & 1)
+            return fail (ctx, "awm_set_sync_tables: entry %d repeats a band in its up or down list", i);
+          seen_up[u >> 5] |= 1u << (u & 31);
+          seen_down[d >> 5] |= 1u << (d & 31);
+        }
+      max_frame = std::max (max_frame, int (entries[i].frame));
+    }
   CK (cudaSetDevice (ctx->device));
   SyncTab& t = ctx->keys[key_slot].sync[mode];
   CK (t.ent.reserve (sizeof (awm_sync_entry) * n_entries));
@@ -709,8 +730,6 @@ awm_set_sync_tables (awm_ctx *ctx, int key_slot, int mode, const awm_sync_entry 
   CK (cudaMemcpyAsync (t.ent.p, entries, sizeof (awm_sync_entry) * n_entries, cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaMemcpyAsync (t.off.p, bit_offsets, sizeof (int) * (n_bits + 1), cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaStreamSynchronize (ctx->stream));
-  if (n_bits > 6)
-    return fail (ctx, "awm_set_sync_tables: at most 6 sync bits are supported");
   /* k_sync_approx walks all entries in ascending frame order (per-bit order is kept: frames are sorted inside a bit) */
   std::vector<ApproxEntry> sorted (n_entries);
   {
@@ -756,6 +775,7 @@ awm_set_sync_tables (awm_ctx *ctx, int key_slot, int mode, const awm_sync_entry 
   t.n_groups = int (group_end.size());
   t.n_ent = n_entries;
   t.n_bits = n_bits;
+  t.max_frame = max_frame;
   t.h_ent.assign (entries, entries + n_entries);
   t.h_off.assign (bit_offsets, bit_offsets + n_bits + 1);
   return 0;
@@ -1562,11 +1582,15 @@ approx_launch (awm_ctx *ctx, awm_ctx::ApproxSlot& s, int key_slot, int mode, uin
     return fail (ctx, "awm_sync_approx: no PCM bound");
   CK (cudaSetDevice (ctx->device));
   const int total = fpb * (mode == AWM_MODE_CLIP ? 2 : 1);
+  /* start frame s reads frame s + entry frame: past the block it would read the scores of a later start frame, or another entry's row */
+  if (t.max_frame >= total)
+    return fail (ctx, "awm_sync_approx: sync entry frame %d is not inside the %d frames of a search (frames_per_block %d)", t.max_frame, total, fpb);
   const long long fc = (long long) (ctx->pcm_frames / kFrame);           // frame_count (wav_data)
   const long long n_out = fc > 0 ? fc - 1 : 0;                           // sync_fft_parallel: frame_count - 1 frames per shift
   const long long n_starts = fc - total - 1 > 0 ? fc - total - 1 : 0;    // (start + total) * n_bands < fft_db.size()
   *n_scores = size_t (n_starts) * 4;
   s.n_scores = 0;
+  s.n_have = 0;
   s.pcm = ctx->pcm;
   s.pcm_frames = ctx->pcm_frames;
   s.pcm_ch = ctx->pcm_ch;
@@ -1683,6 +1707,8 @@ approx_launch (awm_ctx *ctx, awm_ctx::ApproxSlot& s, int key_slot, int mode, uin
     LAUNCH_CHECK ("k_local_mean");
   }
   s.n_scores = size_t (n_starts) * 4;
+  s.n_have = n_out;
+  s.ld_have = ld;
   CK (cudaEventRecord (s.done, ctx->stream));
   if (scores_out)
     {
@@ -1748,6 +1774,23 @@ awm_sync_use_slot (awm_ctx *ctx, int slot, size_t *n_scores)
   ctx->pcm_ch = s.pcm_ch;
   if (n_scores)
     *n_scores = s.n_scores;
+  return 0;
+}
+
+int
+awm_sync_have (awm_ctx *ctx, unsigned char *out, size_t max, size_t *n_frames)
+{
+  if (!n_frames || (max && !out))
+    return fail (ctx, "awm_sync_have: bad arguments");
+  const awm_ctx::ApproxSlot& s = ctx->aslot[ctx->cur_aslot];
+  *n_frames = size_t (s.n_have);
+  if (!s.n_have || !max)
+    return 0;
+  if (max < size_t (4) * s.n_have)
+    return fail (ctx, "awm_sync_have: out too small (%zu < %lld)", max, 4 * s.n_have);
+  CK (cudaSetDevice (ctx->device));
+  CK (cudaMemcpy2DAsync (out, size_t (s.n_have), s.have.p, size_t (s.ld_have), size_t (s.n_have), 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK (cudaStreamSynchronize (ctx->stream));
   return 0;
 }
 

@@ -1007,11 +1007,11 @@ int
 awmh_stage_select (const awm_search_score *peaks, size_t n, double floor_q, int clip_mode, awm_search_score *out, size_t max_out, size_t *n_out, int *complete)
 {
   std::vector<awm_search_score> sel;
-  *complete = select_candidates_from_peaks (peaks, n, floor_q, Params::sync_threshold2 * 0.75, sel) > 0 ? 1 : 0;
+  const size_t n_max = clip_mode ? std::max (Params::get_n_best, 5) : 0;
+  *complete = select_candidates_from_peaks (peaks, n, floor_q, Params::sync_threshold2 * 0.75, sel, n_max) > 0 ? 1 : 0;
   if (clip_mode)
     {
       std::sort (sel.begin(), sel.end(), [] (const awm_search_score& a, const awm_search_score& b) { return fabs (a.raw_quality - a.local_mean) > fabs (b.raw_quality - b.local_mean); });
-      const size_t n_max = std::max (Params::get_n_best, 5);
       if (sel.size() > n_max)
         sel.resize (n_max);
     }

@@ -76,6 +76,13 @@ select_candidates_reference_order (const SearchScore *sc, size_t n, double thres
   select_from_maxima_reference_order (maxima, threshold, out);
 }
 
+/* scores sorted by descending |q - mean|: equal scores on both sides of a cut after the first n */
+bool
+tie_at (const vector<SearchScore>& sorted, size_t n)
+{
+  return n && sorted.size() > n && abs_quality (sorted[n - 1]) == abs_quality (sorted[n]);
+}
+
 } // namespace
 
 /* Candidate selection on a list of local maxima (sorted by index) that is complete above `floor_q`
@@ -85,9 +92,12 @@ select_candidates_reference_order (const SearchScore *sc, size_t n, double thres
  * would need a peak at or below the floor, every peak the reference would select has been seen.
  * Returns 1: `out` is final.  0: the list was too short, ask again with a lower floor.  -1: peaks of EQUAL strength sit on both
  * sides of the n-best cut, which of them the reference keeps is decided by std::sort on the full list of maxima -- ask for all
- * maxima (floor < 0); with a complete list the reference's order of operations is followed literally. */
+ * maxima (floor < 0); with a complete list the reference's order of operations is followed literally.
+ * truncate_n > 0: the caller keeps only the truncate_n strongest of `out` (CLIP mode).  Which of several EQUAL scores on that cut
+ * survive is again decided by std::sort, over the reference's own sequence, so a tie there also returns -1. */
 int
-select_candidates_from_peaks (const awm_search_score *peaks, size_t n, double floor_q, double threshold, vector<awm_search_score>& out)
+select_candidates_from_peaks (const awm_search_score *peaks, size_t n, double floor_q, double threshold, vector<awm_search_score>& out,
+                              size_t truncate_n)
 {
   constexpr int    mask_distance = local_mean_distance + 3;
   constexpr double mask_factor   = 3;
@@ -142,7 +152,7 @@ select_candidates_from_peaks (const awm_search_score *peaks, size_t n, double fl
                 if (!masked (order[kk]))
                   return -1;
             }
-          return 1;
+          return tie_at (out, truncate_n) ? -1 : 1;
         }
       if (q <= floor_q)
         return 0;                               // peaks at or below the floor may be missing from the list
@@ -150,7 +160,9 @@ select_candidates_from_peaks (const awm_search_score *peaks, size_t n, double fl
         out.push_back (pk[i]);
     }
   /* list exhausted: it held only the peaks above the floor; final if n_best unmasked peaks lie above it */
-  return int (out.size()) >= Params::get_n_best ? 1 : 0;
+  if (int (out.size()) < Params::get_n_best)
+    return 0;
+  return tie_at (out, truncate_n) ? -1 : 1;
 }
 
 namespace {
@@ -158,7 +170,7 @@ namespace {
 /* the local maxima come from the GPU (awm_sync_peaks); only those above a floor are transferred, the floor is lowered
  * until the selection is complete */
 bool
-select_candidates_gpu (awm_ctx *ctx, double threshold, vector<SearchScore>& out)
+select_candidates_gpu (awm_ctx *ctx, double threshold, size_t truncate_n, vector<SearchScore>& out)
 {
   static SearchScore *peaks = nullptr;
   static const size_t max_peaks = 1 << 18;    // a 30 minute chunk has at most 150 584 local maxima
@@ -174,14 +186,14 @@ select_candidates_gpu (awm_ctx *ctx, double threshold, vector<SearchScore>& out)
         return false;
       if (n > max_peaks)
         return false;                             // caller falls back to the full score list
-      const int r = select_candidates_from_peaks (peaks, n, floor_q, threshold, out);
+      const int r = select_candidates_from_peaks (peaks, n, floor_q, threshold, out, truncate_n);
       if (r > 0)
         return true;
       if (r < 0 && floor_q >= 0)                  // a tie on the cut: only the complete list of maxima decides it
         {
           if (awm_sync_peaks (ctx, -1.0, peaks, max_peaks, &n) || n > max_peaks)
             return false;
-          return select_candidates_from_peaks (peaks, n, -1.0, threshold, out) > 0;
+          return select_candidates_from_peaks (peaks, n, -1.0, threshold, out, truncate_n) > 0;
         }
     }
   return false;
@@ -301,7 +313,8 @@ SyncFinder::search (const vector<Key>& key_list, size_t n_frames, int n_channels
           else
             ok = awm_sync_approx (ctx, slot, amode, wav_first, wav_last, Params::water_delta, nullptr, 0, &n_scores) == 0;
           /* the scores stay on the device; normally only the peaks that matter come back */
-          gpu_selected = ok && n_scores && select_candidates_gpu (ctx, Params::sync_threshold2 * 0.75, scores);
+          const size_t truncate_n = mode == Mode::CLIP ? std::max (Params::get_n_best, 5) : 0;
+          gpu_selected = ok && n_scores && select_candidates_gpu (ctx, Params::sync_threshold2 * 0.75, truncate_n, scores);
           if (gpu_selected)
             n_scores = 0;                         // nothing else to fetch
           if (ok && n_scores > all_cap)

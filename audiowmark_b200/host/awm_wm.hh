@@ -96,6 +96,7 @@ public:
 
 /* stage functions of SyncFinder::search / BlockDecoder::run, used by get_watermark_buffer and by the frame-balanced
  * multi-GPU driver (audiowmark_b200/sharding.py), which runs the GPU stages on slices of a chunk on different ranks */
-int  select_candidates_from_peaks (const awm_search_score *peaks, size_t n, double floor_q, double threshold, std::vector<awm_search_score>& out);
+int  select_candidates_from_peaks (const awm_search_score *peaks, size_t n, double floor_q, double threshold, std::vector<awm_search_score>& out,
+                                  size_t truncate_n = 0);
 void select_final_scores (std::vector<awm_search_score>& scores, std::vector<SyncFinder::Score>& out);
 

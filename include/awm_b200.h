@@ -85,7 +85,10 @@ int awm_fft_c2r (awm_ctx *ctx, const float *in, float *out, size_t count, int n)
  * embed : FrameMod table of init_frame_mod_vec (src/wmadd.cc:148-162): uint8 [2 (A,B)][frames_per_block][101],
  *         0 keep / 1 up / 2 down
  * sync  : SyncFinder::get_sync_bits (src/syncfinder.cc:30-77) flattened bit-major; bit b owns
- *         entries bit_offsets[b] .. bit_offsets[b+1]-1, entries sorted by frame inside a bit
+ *         entries bit_offsets[b] .. bit_offsets[b+1]-1, entries sorted by frame inside a bit; at most 6 bits,
+ *         offsets non-decreasing, bands < 81 and no band twice in one entry's up (or down) list, else the call
+ *         fails and the slot keeps its previous table.  A search fails if an entry frame is not below
+ *         frames_per_block (twice that in CLIP mode)
  * mix   : gen_mix_entries (src/wmcommon.cc:179-202) and the bit order permutation of
  *         randomize_bit_order (src/wmcommon.hh:165-185): out[bit_order[i]] = in[i] on decode
  * key_slot selects one of AWM_MAX_KEYS table sets (audiowmark get accepts several --key options).
@@ -297,6 +300,11 @@ int awm_sync_approx (awm_ctx *ctx, int key_slot, int mode, uint64_t wav_first, u
  * awm_sync_approx itself works on the current slot. */
 int awm_sync_approx_enqueue (awm_ctx *ctx, int slot, int key_slot, int mode, uint64_t wav_first, uint64_t wav_last, double water_delta);
 int awm_sync_use_slot (awm_ctx *ctx, int slot, size_t *n_scores);
+
+/* The frames the last search of the current approx slot computed: out[shift][frame] = 1 where sync_fft analysed the frame, 0 where it
+ * lies in leading / trailing digital silence (CLIP mode); 4 rows of *n_frames (frame_count - 1) each.  With max = 0 only *n_frames is
+ * returned.  For tests of the spectrogram kernels. */
+int awm_sync_have (awm_ctx *ctx, unsigned char *out, size_t max, size_t *n_frames);
 
 /* awm_sync_peaks = sync_select_local_maxima (src/syncfinder.cc:258-281) on the score list of the current
  * approx slot (kept on the device), restricted to peaks with |raw_quality - local_mean| > min_abs_quality:
