@@ -34,6 +34,7 @@ EXPORTS = [
     "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch", "awm_batch_rates_validate", "awm_embed_batch_rates",
     "awm_batch_offsets_validate", "awm_embed_batch_offsets", "awm_batch_rates_offsets_validate", "awm_embed_batch_rates_offsets",
     "awm_set_embed_roles_keys", "awm_get_embed_roles_keys", "awm_batch_keys_validate", "awm_embed_batch_keys",
+    "awm_speed_mags", "awm_resampler_cache",
 ]
 
 _lib = None
@@ -402,3 +403,20 @@ class Context:
                                          ctypes.c_double(seconds), _ptr(centers), ctypes.c_int(len(centers)), _ptr(rel), ctypes.c_int(rel.shape[1]),
                                          ctypes.c_double(water_delta), _ptr(out)))
         return out
+
+    def speed_mags(self, center: int) -> np.ndarray:
+        """awm_speed_mags: the MagMatrix of centre `center` of the last speed_scan, float32 [n_entries][rows][2] (umag, dmag), entries in
+        table order"""
+        rows, n_ent = ctypes.c_int(), ctypes.c_int()
+        self._ck(self.lib.awm_speed_mags(self.h, ctypes.c_int(center), None, ctypes.c_size_t(0), ctypes.byref(rows), ctypes.byref(n_ent)))
+        out = np.zeros((n_ent.value, rows.value, 2), np.float32)
+        if out.size:
+            self._ck(self.lib.awm_speed_mags(self.h, ctypes.c_int(center), _ptr(out), ctypes.c_size_t(out.size // 2), ctypes.byref(rows),
+                                             ctypes.byref(n_ent)))
+        return out
+
+    def resampler_cache(self) -> tuple[int, int]:
+        """awm_resampler_cache: (filter tables held, tables held before the cache is emptied)"""
+        size, cap = ctypes.c_size_t(), ctypes.c_size_t()
+        self._ck(self.lib.awm_resampler_cache(self.h, ctypes.byref(size), ctypes.byref(cap)))
+        return size.value, cap.value

@@ -19,7 +19,9 @@
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <algorithm>
+#include <cmath>
 #include <map>
+#include <set>
 #include <thread>
 #include <limits.h>
 #include <math.h>
@@ -207,6 +209,8 @@ struct awm_ctx
   DevBuf rs_in, rs_out, rs_jobs, pcm_rs;
   const float *saved_pcm = nullptr; size_t saved_frames = 0; int saved_ch = 0; bool pushed = false;
   DevBuf win512, sp_clip, sp_sub, sp_mags, sp_mag_jobs, sp_cmp_jobs, sp_best;
+  std::vector<MagJob> sp_last;                                   // the MagMatrix of every centre of the last scan (awm_speed_mags)
+  int sp_last_ent = 0;
 };
 
 namespace {
@@ -2571,8 +2575,13 @@ launch_resample (awm_ctx *ctx, const std::vector<ResampleJob>& jobs, int channel
   CK (cudaMemcpyAsync (ctx->rs_jobs.p, jobs.data(), jobs.size() * sizeof (ResampleJob), cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaStreamSynchronize (ctx->stream));             /* jobs is a caller-owned host vector */
   const dim3 grid (unsigned (std::min<long long> ((max_out + 255) / 256, 1 << 20)), unsigned (jobs.size()));
+  /* float2 loads and stores only where every job's input and output are 8-byte aligned (a device clip may start at any float);
+   * k_resample<0> produces the same bits, resample_dot and resample_dot2 share the arithmetic */
+  bool aligned8 = true;
+  for (const auto& j : jobs)
+    aligned8 = aligned8 && uintptr_t (j.in) % 8 == 0 && uintptr_t (j.out) % 8 == 0;
   PROF (ctx);
-  if (channels == 2)
+  if (channels == 2 && aligned8)
     k_resample<2><<<grid, 256, 0, ctx->stream>>> (ctx->rs_jobs.as<ResampleJob>(), channels);
   else if (channels == 1)
     k_resample<1><<<grid, 256, 0, ctx->stream>>> (ctx->rs_jobs.as<ResampleJob>(), channels);
@@ -3099,11 +3108,88 @@ awm_speed_scan (awm_ctx *ctx, int key_slot, const float *clip, size_t clip_frame
   if (t.n_ent > kCmpMaxEntries)
     return fail (ctx, "awm_speed_scan: %d sync entries exceed the kernel limit %d", t.n_ent, kCmpMaxEntries);
   const size_t n_jobs = size_t (n_centers) * n_relative;
+  if (n_jobs > 65535)
+    return fail (ctx, "awm_speed_scan: %d centres x %d relative speeds = %zu jobs exceed the limit 65535", n_centers, n_relative, n_jobs);
+  for (size_t i = 0; i < n_jobs; i++)
+    if (!(std::isfinite (relative_speeds[i]) && relative_speeds[i] > 0))
+      return fail (ctx, "awm_speed_scan: relative speed %g (job %zu) is not finite and > 0", relative_speeds[i], i);
   for (size_t i = 0; i < n_jobs; i++)
     quality_out[i] = 0;
+  ctx->sp_last.clear();
+  ctx->sp_last_ent = t.n_ent;
   if (!n_jobs)
     return 0;
   CK (cudaSetDevice (ctx->device));
+  /* geometry per centre: resample_ratio_truncate (in_data, center / 2, ..., seconds / center), src/wmspeed.cc:206 + src/resample.cc:100-125 */
+  std::vector<ResampleJob> rj (n_centers);
+  std::vector<MagJob> mj (n_centers);
+  std::vector<CmpJob> cj (n_jobs);
+  size_t sub_total = 0, mag_total = 0;
+  int max_rows = 0;
+  for (int c = 0; c < n_centers; c++)
+    {
+      const double ratio = centers[c] / 2;
+      if (!resample_ratio_ok (ratio))
+        return fail (ctx, "awm_speed_scan: centre %g not supported", centers[c]);
+      const double max_in_seconds = seconds / centers[c];
+      size_t in_trunc = clip_frames;
+      if (max_in_seconds > 0)
+        in_trunc = std::min<size_t> (in_trunc, size_t (lrint (sample_rate * max_in_seconds)));
+      const long long n_sub = lrint (double (in_trunc) * ratio);
+      const int rows = n_sub > kSpeedFrame ? int ((n_sub - kSpeedFrame + kSpeedHop - 1) / kSpeedHop) : 0;
+      rj[c].n_in = (long long) in_trunc;
+      rj[c].n_stop = rj[c].n_in;
+      rj[c].n_out = n_sub;
+      rj[c].step = 1.0 / ratio;
+      mj[c].n_sub = n_sub;
+      mj[c].rows = rows;
+      sub_total += size_t (n_sub) * channels;
+      mag_total += size_t (rows) * t.n_ent;
+      max_rows = std::max (max_rows, rows);
+    }
+  /* SpeedSync::compare: offsets -pad_start .. -1, pad_start = one block + one frame in search steps (src/wmspeed.cc:331) */
+  const int pad_start = fpb * 4 + 4;
+  for (int c = 0; c < n_centers; c++)
+    for (int r = 0; r < n_relative; r++)
+      {
+        CmpJob& J = cj[size_t (c) * n_relative + r];
+        const double rs = relative_speeds[size_t (c) * n_relative + r];
+        J.rows = mj[c].rows;
+        J.inv = 1 / rs;                              /* relative_speed_inv, src/wmspeed.cc:274 */
+        J.off_scale = (1 << 16) / rs;                /* src/wmspeed.cc:341 */
+        /* the 16.16 contract of k_speed_compare: the most negative offset and every frame offset below fo_cut fit in 31 bits */
+        const double off_min = double (-pad_start) * J.off_scale;
+        if (!(off_min > -2147483647.0))
+          return fail (ctx, "awm_speed_scan: relative speed %g: start offsets need more than 31 bits in 16.16", rs);
+        J.fo_cut = 65536.0 * J.rows - double (int (off_min));
+        if (J.fo_cut <= 2147483648.0)                /* every frame offset below fo_cut fits (always so for scans of <= 50 s) */
+          continue;
+        for (int B = 0; B < 3; B++)
+          for (const auto& e : t.h_ent)
+            {
+              const double f = (double ((B * (long long) fpb + e.frame) * 4) * J.inv + 0.5) * 65536.0;
+              if (f < J.fo_cut && f >= 2147483648.0)
+                return fail (ctx, "awm_speed_scan: relative speed %g, %d rows: an entry of block %d at frame %d needs a 16.16 offset of more "
+                             "than 31 bits", rs, J.rows, B, int (e.frame));
+            }
+      }
+  /* every filter table this scan needs, fetched after making room for all new ones at once: coef_table empties a full cache,
+   * which would free the tables of the centres already collected.  Making room may empty the cache, after which every distinct
+   * centre of the call is fetched anew, so all of them (not only the new ones) must fit: then no fetch below empties it again */
+  {
+    std::set<double> ratios;
+    size_t n_new = 0;
+    for (int c = 0; c < n_centers; c++)
+      if (ratios.insert (centers[c] / 2).second && !ctx->coef_cache.count (std::make_pair (centers[c] / 2, 16)))
+        n_new++;
+    if (ratios.size() > kCoefCacheCap)
+      return fail (ctx, "awm_speed_scan: %zu distinct centres exceed the resampler table cache (%zu)", ratios.size(), kCoefCacheCap);
+    if (coef_cache_room (ctx, n_new))
+      return 1;
+  }
+  for (int c = 0; c < n_centers; c++)
+    if (coef_table (ctx, centers[c] / 2, 16, &rj[c].coef, &rj[c].h))
+      return 1;
   if (!ctx->win512.p)
     {
       /* FFTAnalyzer::gen_normalized_window (sub_frame_size), src/wmcommon.cc:68-89 */
@@ -3127,38 +3213,8 @@ awm_speed_scan (awm_ctx *ctx, int key_slot, const float *clip, size_t clip_frame
       CK (cudaMemcpyAsync (ctx->sp_clip.p, clip, clip_frames * channels * sizeof (float), cudaMemcpyHostToDevice, ctx->stream));
       d_clip = ctx->sp_clip.as<float>();
     }
-  /* geometry per centre: resample_ratio_truncate (in_data, center / 2, ..., seconds / center), src/wmspeed.cc:206 + src/resample.cc:100-125 */
-  std::vector<ResampleJob> rj (n_centers);
-  std::vector<MagJob> mj (n_centers);
-  std::vector<CmpJob> cj (n_jobs);
-  size_t sub_total = 0, mag_total = 0;
-  int max_rows = 0;
   for (int c = 0; c < n_centers; c++)
-    {
-      const double ratio = centers[c] / 2;
-      const float *coef;
-      int h;
-      if (coef_table (ctx, ratio, 16, &coef, &h))
-        return 1;
-      const double max_in_seconds = seconds / centers[c];
-      size_t in_trunc = clip_frames;
-      if (max_in_seconds > 0)
-        in_trunc = std::min<size_t> (in_trunc, size_t (lrint (sample_rate * max_in_seconds)));
-      const long long n_sub = lrint (double (in_trunc) * ratio);
-      const int rows = n_sub > kSpeedFrame ? int ((n_sub - kSpeedFrame + kSpeedHop - 1) / kSpeedHop) : 0;
-      rj[c].in = d_clip;
-      rj[c].n_in = (long long) in_trunc;
-      rj[c].n_stop = rj[c].n_in;
-      rj[c].n_out = n_sub;
-      rj[c].step = 1.0 / ratio;
-      rj[c].h = h;
-      rj[c].coef = coef;
-      mj[c].n_sub = n_sub;
-      mj[c].rows = rows;
-      sub_total += size_t (n_sub) * channels;
-      mag_total += size_t (rows) * t.n_ent;
-      max_rows = std::max (max_rows, rows);
-    }
+    rj[c].in = d_clip;
   CK (ctx->sp_sub.reserve (std::max<size_t> (sub_total, 1) * sizeof (float)));
   CK (ctx->sp_mags.reserve (std::max<size_t> (mag_total, 1) * sizeof (float2)));
   {
@@ -3171,14 +3227,7 @@ awm_speed_scan (awm_ctx *ctx, int key_slot, const float *clip, size_t clip_frame
         so += size_t (rj[c].n_out) * channels;
         mo += size_t (mj[c].rows) * t.n_ent;
         for (int r = 0; r < n_relative; r++)
-          {
-            CmpJob& J = cj[size_t (c) * n_relative + r];
-            const double rs = relative_speeds[size_t (c) * n_relative + r];
-            J.mags = mj[c].mags;
-            J.rows = mj[c].rows;
-            J.inv = 1 / rs;                              /* relative_speed_inv, src/wmspeed.cc:274 */
-            J.off_scale = (1 << 16) / rs;                /* src/wmspeed.cc:341 */
-          }
+          cj[size_t (c) * n_relative + r].mags = mj[c].mags;
       }
   }
   if (launch_resample (ctx, rj, channels))
@@ -3197,8 +3246,6 @@ awm_speed_scan (awm_ctx *ctx, int key_slot, const float *clip, size_t clip_frame
       k_speed_mags<<<grid, kMagWarps * 32, kMagSmemBytes, ctx->stream>>> (ctx->sp_mag_jobs.as<MagJob>(), channels, t.ent.as<awm_sync_entry>(), t.n_ent,
                                                                           ctx->tw.as<float2>(), ctx->win512.as<float>());
       LAUNCH_CHECK ("k_speed_mags");
-      /* SpeedSync::compare: offsets -pad_start .. -1, pad_start = one block + one frame in search steps (src/wmspeed.cc:331) */
-      const int pad_start = fpb * 4 + 4;
       const double norm_div = water_delta < 0.080 ? water_delta : 0.080;
       const dim3 cgrid (unsigned ((pad_start + 255) / 256), unsigned (n_jobs));
       PROF (ctx);
@@ -3209,5 +3256,35 @@ awm_speed_scan (awm_ctx *ctx, int key_slot, const float *clip, size_t clip_frame
   static_assert (sizeof (double) == sizeof (unsigned long long), "quality bits");
   CK (cudaMemcpyAsync (quality_out, ctx->sp_best.p, n_jobs * sizeof (double), cudaMemcpyDeviceToHost, ctx->stream));
   CK (cudaStreamSynchronize (ctx->stream));
+  ctx->sp_last = mj;
+  return 0;
+}
+
+int
+awm_speed_mags (awm_ctx *ctx, int center, float *out, size_t max, int *rows, int *n_entries)
+{
+  if (!rows || !n_entries || center < 0 || size_t (center) >= ctx->sp_last.size())
+    return fail (ctx, "awm_speed_mags: bad arguments (centre %d of %zu)", center, ctx->sp_last.size());
+  const MagJob& m = ctx->sp_last[center];
+  *rows = m.rows;
+  *n_entries = ctx->sp_last_ent;
+  const size_t n = size_t (m.rows) * ctx->sp_last_ent;
+  if (!out || !n)
+    return 0;
+  if (max < n)
+    return fail (ctx, "awm_speed_mags: out too small (%zu < %zu)", max, n);
+  CK (cudaSetDevice (ctx->device));
+  CK (cudaMemcpyAsync (out, m.mags, n * sizeof (float2), cudaMemcpyDeviceToHost, ctx->stream));
+  CK (cudaStreamSynchronize (ctx->stream));
+  return 0;
+}
+
+int
+awm_resampler_cache (awm_ctx *ctx, size_t *size, size_t *cap)
+{
+  if (!size || !cap)
+    return fail (ctx, "awm_resampler_cache: bad arguments");
+  *size = ctx->coef_cache.size();
+  *cap = kCoefCacheCap;
   return 0;
 }

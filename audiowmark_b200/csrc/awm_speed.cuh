@@ -316,15 +316,22 @@ struct CmpJob
   int           rows;
   double        inv;         // 1 / relative_speed
   double        off_scale;   // 65536 / relative_speed
+  double        fo_cut;      // 65536 rows - (most negative offset): a frame offset at or above it lands past the last row for
+                             // every offset of the job
 };
 
 constexpr int kCmpMaxEntries = 1024;
+constexpr int kCmpNever = -1;              // frame offset of an entry that lands in no row: offset + kCmpNever < 0 for every offset
 
 // thread = one start offset (CmpState, src/wmspeed.cc:118-122).  The reference walks the frame-sorted entry list once per
 // block and scatters into six per-bit accumulators; the per-bit sums only depend on the order inside a bit, so here each
 // bit is summed on its own (entries are stored bit major, frame sorted inside a bit: the layout of awm_set_sync_tables).
 // The begin / end iterators of compare_bits are the index tests s >= 0 and (s >> 16) < rows: offsets and frame offsets
 // both grow monotonically.
+// 16.16 contract: offsets and frame offsets are the reference's truncated doubles, and an entry counts at row (offset + fo) >> 16
+// exactly as in integer arithmetic of unbounded width.  A frame offset at or above fo_cut (it can never index a row) is stored
+// as kCmpNever, which fails the s >= 0 test; awm_speed_scan refuses jobs whose offsets or remaining frame offsets need more
+// than 31 bits, so s = offset + fo never wraps.
 __global__ void __launch_bounds__ (256)
 k_speed_compare (const CmpJob *__restrict__ jobs, const awm_sync_entry *__restrict__ ent, const int *__restrict__ bit_off, int n_bits,
                  int n_ent, int frames_per_block, int pad_start, double norm_div, unsigned long long *__restrict__ best)
@@ -335,7 +342,8 @@ k_speed_compare (const CmpJob *__restrict__ jobs, const awm_sync_entry *__restri
     {
       const int B = idx / n_ent, e = idx - B * n_ent;
       const int v = (B * frames_per_block + int (ent[e].frame)) * 4;             // steps_per_frame = 4
-      fo[idx] = int (__dmul_rn (__dadd_rn (__dmul_rn (double (v), J.inv), 0.5), 65536.0));   // src/wmspeed.cc:280
+      const double f = __dmul_rn (__dadd_rn (__dmul_rn (double (v), J.inv), 0.5), 65536.0);   // src/wmspeed.cc:280
+      fo[idx] = f < J.fo_cut ? int (f) : kCmpNever;
     }
   __syncthreads();
   const int o = blockIdx.x * blockDim.x + threadIdx.x;

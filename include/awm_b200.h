@@ -384,10 +384,21 @@ int awm_is_device_pointer (const void *p);
  * scored for n_relative relative speeds (relative_speeds[c * n_relative + r] = pow (step, p) * speed / centre, :173).
  * quality_out[c * n_relative + r] = Score::quality of that compare() call (0 if no offset had data).
  * Uses the BLOCK mode sync table of key_slot (awm_set_sync_tables) and frames_per_block of awm_set_mix_tables.
+ * Refused before any work: relative speeds that are not finite and > 0, more than 65535 (centre, relative speed) pairs, more
+ * distinct centres than the resampler table cache holds (1024), and jobs whose 16.16 start offsets, or the frame offsets of
+ * entries that can still land inside the MagMatrix, do not fit in 31 bits (the reference's int arithmetic would overflow; the
+ * CLI's scans of at most 50 s never get there).  Entries that land past the last row for every start offset are skipped.
  */
 int awm_speed_scan (awm_ctx *ctx, int key_slot, const float *clip, size_t clip_frames, int channels, int sample_rate,
                     double seconds, const double *centers, int n_centers, const double *relative_speeds, int n_relative,
                     double water_delta, double *quality_out);
+
+/* inspection of the last awm_speed_scan: *rows and *n_entries = shape of the MagMatrix of centre `center`; with out, the matrix
+ * (float2 (umag, dmag) [n_entries][rows], entries in table order) is copied there (max = capacity in float2) */
+int awm_speed_mags (awm_ctx *ctx, int center, float *out, size_t max, int *rows, int *n_entries);
+
+/* resampler filter tables: how many the context holds and how many it keeps before it empties the cache */
+int awm_resampler_cache (awm_ctx *ctx, size_t *size, size_t *cap);
 
 /* ---- multi-GPU exchange for the sharded `get` (one process per GPU) ------------------------------------------------------
  * The reference has no counterpart: its thread pool shares one address space.  Here the ranks of a job exchange the small
