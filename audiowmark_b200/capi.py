@@ -270,6 +270,20 @@ class Context:
                                     ctypes.c_int(limiter_block), ctypes.c_float(limiter_ceiling), snr if want_snr else None))
         return (pcm_out, (snr[0], snr[1])) if want_snr else pcm_out
 
+    def embed_s16(self, pcm_in, pcm_out=None, n_frames=None, channels=None, first_frame_number=0, frames_pad_start=250,
+                  water_delta=0.01, limiter_block=44100, limiter_ceiling=0.99, want_snr=False):
+        """awm_embed_s16: embed as awm_embed between 16 bit buffers (int16 numpy arrays or device pointers with sizes given)"""
+        if isinstance(pcm_in, np.ndarray):
+            pcm_in = np.ascontiguousarray(pcm_in, np.int16)
+            n_frames, channels = pcm_in.shape
+            if pcm_out is None:
+                pcm_out = np.empty_like(pcm_in)
+        snr = (ctypes.c_double * 2)()
+        self._ck(self.lib.awm_embed_s16(self.h, _ptr(pcm_in), _ptr(pcm_out), ctypes.c_size_t(n_frames), ctypes.c_int(channels),
+                                        ctypes.c_uint64(first_frame_number), ctypes.c_int(frames_pad_start), ctypes.c_double(water_delta),
+                                        ctypes.c_int(limiter_block), ctypes.c_float(limiter_ceiling), snr if want_snr else None))
+        return (pcm_out, (snr[0], snr[1])) if want_snr else pcm_out
+
     # ---- sync
     def sync_approx(self, key_slot=0, mode=MODE_BLOCK, wav_first=0, wav_last=None, water_delta=0.01) -> np.ndarray:
         if wav_last is None:

@@ -599,8 +599,12 @@ awm_set_embed_tables (awm_ctx *ctx, const uint8_t *frame_mod_ab, int frames_per_
 {
   if (!frame_mod_ab || frames_per_block <= 0)
     return fail (ctx, "awm_set_embed_tables: bad arguments");
-  CK (cudaSetDevice (ctx->device));
   const size_t bytes = size_t (2) * frames_per_block * (kMaxBand + 1);
+  for (size_t i = 0; i < bytes; i++)               /* the kernels read bins kMinBand .. kMaxBand, and 1 as up, anything else as down */
+    if (frame_mod_ab[i] > 2 || (frame_mod_ab[i] && int (i % (kMaxBand + 1)) < kMinBand))
+      return fail (ctx, "awm_set_embed_tables: entry %zu (row %zu, bin %d) is %d: entries are 0 keep, 1 up, 2 down, and bins below %d are kept",
+                   i, i / (kMaxBand + 1), int (i % (kMaxBand + 1)), int (frame_mod_ab[i]), kMinBand);
+  CK (cudaSetDevice (ctx->device));
   CK (ctx->frame_mod.reserve (bytes));
   CK (cudaMemcpyAsync (ctx->frame_mod.p, frame_mod_ab, bytes, cudaMemcpyHostToDevice, ctx->stream));
   CK (cudaStreamSynchronize (ctx->stream));
@@ -839,7 +843,7 @@ pcm_bind_any (awm_ctx *ctx, const void *pcm_v, bool s16, size_t n_frames, int ch
         {
           const long long n_val = (long long) (n_frames * channels);
           PROF (ctx);
-          k_s16_to_f32<<<unsigned (((n_val + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (hit->buf16.as<int16_t>(), hit->buf.as<float>(), n_val);
+          s16_to_f32_kernel (hit->buf16.as<int16_t>(), hit->buf.as<float>())<<<unsigned (((n_val + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (hit->buf16.as<int16_t>(), hit->buf.as<float>(), n_val);
           LAUNCH_CHECK ("k_s16_to_f32");
         }
       ctx->pcm = hit->buf.as<float>();
@@ -870,7 +874,7 @@ pcm_bind_any (awm_ctx *ctx, const void *pcm_v, bool s16, size_t n_frames, int ch
               src16 = ctx->pcm16_own.as<int16_t>();
             }
           PROF (ctx);
-          k_s16_to_f32<<<unsigned (((n_val + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (src16, d + pad_start * channels, n_val);
+          s16_to_f32_kernel (src16, d + pad_start * channels)<<<unsigned (((n_val + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (src16, d + pad_start * channels, n_val);
           LAUNCH_CHECK ("k_s16_to_f32");
         }
       if (pad_end)
@@ -1018,7 +1022,7 @@ awm_pcm_stage_wait (awm_ctx *ctx, size_t n_frames)
       const size_t v0 = f0 * ctx->stage_ch;
       const long long nv = (long long) ((f1 - f0) * ctx->stage_ch);
       PROF (ctx);
-      k_s16_to_f32<<<unsigned (((nv + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (ctx->staged16.as<int16_t>() + v0, ctx->staged.as<float>() + v0, nv);
+      s16_to_f32_kernel (ctx->staged16.as<int16_t>() + v0, ctx->staged.as<float>() + v0)<<<unsigned (((nv + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (ctx->staged16.as<int16_t>() + v0, ctx->staged.as<float>() + v0, nv);
       LAUNCH_CHECK ("k_s16_to_f32");
     }
   return 0;
@@ -1042,6 +1046,21 @@ awm_pcm_device (awm_ctx *ctx, size_t *n_frames, int *channels)
 
 namespace {
 
+/* the arguments every entry point that reaches k_embed* shares.  The table row of a stream's first frame is 2*fpb - frames_pad_start,
+ * which must not be negative.  A 1024-frame span touches at most two limiter blocks (k_embed keeps two peaks, k_embed_strip one
+ * boundary per span), and the pipelined limiter of piece p - 1 runs after piece p's embed, so a block may reach at most half a piece
+ * (AWM_PIECE >= 1024 frames) past its end: limiter_block is 0 (off) or in [AWM_MIN_LIMITER_BLOCK, AWM_MAX_LIMITER_BLOCK]. */
+int
+embed_args_check (awm_ctx *ctx, const char *name, int frames_pad_start, int fpb, int limiter_block)
+{
+  if (frames_pad_start < 0 || frames_pad_start > 2 * fpb)
+    return fail (ctx, "%s: frames_pad_start %d outside [0, 2 * frames_per_block = %d]", name, frames_pad_start, 2 * fpb);
+  if (limiter_block != 0 && (limiter_block < AWM_MIN_LIMITER_BLOCK || limiter_block > AWM_MAX_LIMITER_BLOCK))
+    return fail (ctx, "%s: limiter block %d frames outside [%d, %d] (0 disables the limiter)", name, limiter_block, AWM_MIN_LIMITER_BLOCK,
+                 AWM_MAX_LIMITER_BLOCK);
+  return 0;
+}
+
 /* awm_embed / awm_embed_s16: `s16` selects 16 bit PCM buffers (in16 / out16) that are converted on the device */
 int
 embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frames, int channels,
@@ -1056,6 +1075,11 @@ embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frame
     return fail (ctx, "awm_embed: awm_set_embed_tables has not been called");
   if (channels <= 0 || (n_frames && (!in_v || !out_v)))
     return fail (ctx, "awm_embed: bad arguments");
+  if (embed_args_check (ctx, "awm_embed", frames_pad_start, ctx->embed_fpb, limiter_block))
+    return 1;
+  if (first_frame_number > AWM_MAX_STREAM_FRAMES / kFrame || first_frame_number * kFrame + n_frames > AWM_MAX_STREAM_FRAMES)
+    return fail (ctx, "awm_embed: first_frame_number %llu * 1024 + n_frames %zu exceeds the stream length limit of 2^48 frames",
+                 (unsigned long long) first_frame_number, n_frames);
   if (snr_power)
     snr_power[0] = snr_power[1] = 0;
   if (n_frames == 0)
@@ -1095,7 +1119,7 @@ embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frame
         return 0;
       if (st == ctx->stream)          /* the profile events live on the context stream */
         PROF (ctx);
-      k_s16_to_f32<<<unsigned (((v1 - v0 + 1) / 2 + 255) / 256), 256, 0, st>>> (d_in16 + v0, ctx->emb_in.as<float>() + v0, v1 - v0);
+      s16_to_f32_kernel (d_in16 + v0, ctx->emb_in.as<float>() + v0)<<<unsigned (((v1 - v0 + 1) / 2 + 255) / 256), 256, 0, st>>> (d_in16 + v0, ctx->emb_in.as<float>() + v0, v1 - v0);
       LAUNCH_CHECK ("k_s16_to_f32");
       return 0;
     };
@@ -1105,7 +1129,7 @@ embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frame
         return 0;
       if (st == ctx->stream)
         PROF (ctx);
-      k_f32_to_s16<<<unsigned (((v1 - v0 + 1) / 2 + 255) / 256), 256, 0, st>>> (d_out + v0, d_out16 + v0, v1 - v0);
+      f32_to_s16_kernel (d_out + v0, d_out16 + v0)<<<unsigned (((v1 - v0 + 1) / 2 + 255) / 256), 256, 0, st>>> (d_out + v0, d_out16 + v0, v1 - v0);
       LAUNCH_CHECK ("k_f32_to_s16");
       return 0;
     };
@@ -1147,9 +1171,12 @@ embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frame
   A.win = ctx->win.as<float>();
   A.synth = ctx->synth.as<float>();
   const size_t smem = kEmbedSmem;
-  if (set_smem (ctx, k_embed, smem)) return 1;
-  /* stereo audio in a 16-byte aligned buffer streams through k_embed_strip (awm_embed_strip.cuh); anything else takes k_embed */
-  const bool use_strip = channels == 2 && (reinterpret_cast<uintptr_t> (A.in) & 15) == 0;
+  /* stereo audio in a 16-byte aligned buffer (bulk copies) with an 8-byte aligned output (float2 stores) streams through
+   * k_embed_strip (awm_embed_strip.cuh); anything else takes k_embed, with float2 accesses where both buffers allow them */
+  const uintptr_t in_a = reinterpret_cast<uintptr_t> (A.in), out_a = reinterpret_cast<uintptr_t> (A.out);
+  const auto k_embed_any = ((in_a | out_a) & 7) == 0 ? k_embed<true> : k_embed<false>;
+  if (set_smem (ctx, k_embed_any, smem)) return 1;
+  const bool use_strip = channels == 2 && (in_a & 15) == 0 && (out_a & 7) == 0;
   if (use_strip)
     {
       if (!ctx->n_sms)
@@ -1282,7 +1309,7 @@ embed_any (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_frame
         }
       const unsigned grid = unsigned ((A.frame_end - A.frame_begin + kEmbedTile - 1) / kEmbedTile);
       PROF (ctx);
-      k_embed<<<grid, kEmbedWarps * 32, smem, ctx->stream>>> (A);
+      k_embed_any<<<grid, kEmbedWarps * 32, smem, ctx->stream>>> (A);
       LAUNCH_CHECK ("k_embed");
       if (p > 0 && launch_limiter (p - 1))                     // peaks of the blocks after piece p-1 are final now
         return 1;
@@ -1411,7 +1438,7 @@ batch_images (awm_ctx *ctx, const void *in_v, void *out_v, bool s16, size_t n_va
           d_in16 = ctx->emb_in16.as<int16_t>();
         }
       PROF (ctx);
-      k_s16_to_f32<<<unsigned (((n_values + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (d_in16, ctx->emb_in.as<float>(), (long long) n_values);
+      s16_to_f32_kernel (d_in16, ctx->emb_in.as<float>())<<<unsigned (((n_values + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (d_in16, ctx->emb_in.as<float>(), (long long) n_values);
       LAUNCH_CHECK ("k_s16_to_f32");
     }
   else if (!in_dev)
@@ -1435,7 +1462,7 @@ batch_finish (awm_ctx *ctx, void *out_v, bool s16, size_t n_values, const float 
           d_out16 = ctx->emb_out16.as<int16_t>();
         }
       PROF (ctx);
-      k_f32_to_s16<<<unsigned (((n_values + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (d_out, d_out16, (long long) n_values);
+      f32_to_s16_kernel (d_out, d_out16)<<<unsigned (((n_values + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (d_out, d_out16, (long long) n_values);
       LAUNCH_CHECK ("k_f32_to_s16");
       if (!out_dev)
         CK (cudaMemcpyAsync (out_v, d_out16, n_values * sizeof (int16_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2831,6 +2858,12 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
   auto role_table = [&] (size_t i) { return key_index ? int (key_index[i]) : 0; };
   if ((n_items && (!coded_bits || (sample_rates && !n_emit))) || (n_values && (!in_v || !out_v)) || limiter_ms < 0)
     return fail (ctx, "%s: bad arguments", name);
+  /* the limiter block reaches k_embed_batch only through the items at mark_sample_rate; the others' blocks go to k_limiter_rates */
+  bool any44 = !sample_rates;
+  for (size_t i = 0; i < n_items && !any44; i++)
+    any44 = sample_rates[i] == mark_sample_rate;
+  if (embed_args_check (ctx, name, frames_pad_start, rs.fpb, any44 ? limiter_block44 : 0))
+    return 1;
   if (snr_power)
     std::fill (snr_power, snr_power + 2 * n_items, 0.0);
   if (n_values == 0)

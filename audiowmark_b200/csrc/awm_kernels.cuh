@@ -1154,11 +1154,12 @@ embed_tile (const EmbedArgs& A, long long tile_first, unsigned char *smem, FmRow
     }
 }
 
-__global__ void __launch_bounds__ (kEmbedWarps * 32, 1)
+// VEC2: in and out are both 8-byte aligned (stereo as float2); the caller picks it from the pointers, as k_embed_batch does
+template<bool VEC2> __global__ void __launch_bounds__ (kEmbedWarps * 32, 1)
 k_embed (EmbedArgs A)
 {
   extern __shared__ __align__ (16) unsigned char smem[];
-  embed_tile<true> (A, A.frame_begin + (long long) blockIdx.x * kEmbedTile, smem,
+  embed_tile<VEC2> (A, A.frame_begin + (long long) blockIdx.x * kEmbedTile, smem,
                     [&] (long long r) { return A.frame_mod + (size_t) r * (kMaxBand + 1); });
 }
 

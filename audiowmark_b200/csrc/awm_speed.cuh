@@ -122,12 +122,18 @@ k_resample (const ResampleJob *__restrict__ jobs, int c_dyn)
 // 16 bit PCM <-> float exactly as the reference converts around its float pipeline: reading through libsndfile's int
 // API and scaling by 2^-31 (src/sfinputstream.cc:189-210: a 16 bit sample arrives left justified), writing with
 // float_to_int_clip<32> (src/rawconverter.hh:34-50) and keeping the 16 most significant bits (src/sfoutputstream.cc:148-155).
-// Converting on the device halves the PCIe traffic of 16 bit audio.
-__global__ void
+// Converting on the device halves the PCIe traffic of 16 bit audio.  A thread converts values i and i + 1; VEC: as one short2 /
+// float2 access, which needs in 4-byte and out 8-byte aligned (s16_to_f32_kernel picks it from the pointers), else one at a time.
+template<bool VEC> __global__ void
 k_s16_to_f32 (const int16_t *__restrict__ in, float *__restrict__ out, long long n)
 {
   const long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * 2;
-  if (i + 1 < n)
+  if (!VEC)
+    {
+      for (long long j = i; j < i + 2 && j < n; j++)
+        out[j] = float (int (in[j]) << 16) * (1.0f / 2147483648.0f);
+    }
+  else if (i + 1 < n)
     {
       const short2 v = *reinterpret_cast<const short2 *> (in + i);
       *reinterpret_cast<float2 *> (out + i) = make_float2 (float (int (v.x) << 16) * (1.0f / 2147483648.0f), float (int (v.y) << 16) * (1.0f / 2147483648.0f));
@@ -150,11 +156,17 @@ f32_to_s16 (float f)
   return int16_t (v >> 16);
 }
 
-__global__ void
+// VEC: in 8-byte and out 4-byte aligned (f32_to_s16_kernel), as k_s16_to_f32
+template<bool VEC> __global__ void
 k_f32_to_s16 (const float *__restrict__ in, int16_t *__restrict__ out, long long n)
 {
   const long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * 2;
-  if (i + 1 < n)
+  if (!VEC)
+    {
+      for (long long j = i; j < i + 2 && j < n; j++)
+        out[j] = f32_to_s16 (in[j]);
+    }
+  else if (i + 1 < n)
     {
       const float2 v = *reinterpret_cast<const float2 *> (in + i);
       short2 o;
@@ -164,6 +176,19 @@ k_f32_to_s16 (const float *__restrict__ in, int16_t *__restrict__ out, long long
     }
   else if (i < n)
     out[i] = f32_to_s16 (in[i]);
+}
+
+// the instance of each conversion kernel that the two buffers allow
+inline auto
+s16_to_f32_kernel (const int16_t *in, const float *out)
+{
+  return ((reinterpret_cast<uintptr_t> (in) & 3) | (reinterpret_cast<uintptr_t> (out) & 7)) == 0 ? k_s16_to_f32<true> : k_s16_to_f32<false>;
+}
+
+inline auto
+f32_to_s16_kernel (const float *in, const int16_t *out)
+{
+  return ((reinterpret_cast<uintptr_t> (in) & 7) | (reinterpret_cast<uintptr_t> (out) & 3)) == 0 ? k_f32_to_s16<true> : k_f32_to_s16<false>;
 }
 
 // dst[k] = src[idx[k]]: the sparse sample subset get_clip_locations hashes (src/wmspeed.cc:538-543) when the PCM lives in device memory

@@ -94,6 +94,8 @@ int awm_fft_c2r (awm_ctx *ctx, const float *in, float *out, size_t count, int n)
  * key_slot selects one of AWM_MAX_KEYS table sets (audiowmark get accepts several --key options).
  */
 #define AWM_MAX_KEYS 16
+/* frame_mod_ab: uint8 [2 (A, B)][frames_per_block][101], 0 keep, 1 up, 2 down.  A byte above 2, or a nonzero byte below bin 20
+ * (the kernels mark bins 20 .. 100 only), fails the call and leaves the previous table in place. */
 int awm_set_embed_tables (awm_ctx *ctx, const uint8_t *frame_mod_ab, int frames_per_block);
 int awm_set_sync_tables (awm_ctx *ctx, int key_slot, int mode, const awm_sync_entry *entries, int n_entries,
                          const int *bit_offsets, int n_bits);
@@ -142,7 +144,14 @@ const float *awm_pcm_device (awm_ctx *ctx, size_t *n_frames, int *channels);
  * 1000 / 1000 frames (src/limiter.cc:33-37); limiter_block = 0 disables the limiter
  * (--test-no-limiter).  snr_power (optional, 2 doubles) receives sum(delta^2), sum(orig^2)
  * as --snr accumulates them (src/wmadd.cc:553-563).
+ * The call fails before any work, with a message, unless: frames_pad_start is in [0, 2 * frames_per_block];
+ * first_frame_number * 1024 + n_frames <= AWM_MAX_STREAM_FRAMES; limiter_block is 0 or in [AWM_MIN_LIMITER_BLOCK,
+ * AWM_MAX_LIMITER_BLOCK].  The same frames_pad_start and limiter block rules hold for every batched embed below (for the
+ * *_rates and *_keys calls the block mark_sample_rate * limiter_ms / 1000, when an item is at mark_sample_rate).
+ * in / out may be device buffers at any 4-byte alignment (2-byte for the 16 bit variant).
  */
+#define AWM_MIN_LIMITER_BLOCK 1024          /* a 1024-frame span touches at most two limiter blocks */
+#define AWM_MAX_LIMITER_BLOCK (1 << 18)     /* half of the smallest pipeline piece: a block's peak is final before it is applied */
 int awm_embed (awm_ctx *ctx, const float *in, float *out, size_t n_frames, int channels,
                uint64_t first_frame_number, int frames_pad_start, double water_delta,
                int limiter_block, float limiter_ceiling, double *snr_power);
