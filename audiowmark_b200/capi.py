@@ -35,6 +35,8 @@ EXPORTS = [
     "awm_batch_offsets_validate", "awm_embed_batch_offsets", "awm_batch_rates_offsets_validate", "awm_embed_batch_rates_offsets",
     "awm_set_embed_roles_keys", "awm_get_embed_roles_keys", "awm_batch_keys_validate", "awm_embed_batch_keys",
     "awm_speed_mags", "awm_resampler_cache",
+    "awm_resample_stream_available", "awm_resample_stream_frames", "awm_resample_taps", "awm_resample_range_validate", "awm_resample_range",
+    "awm_device_alloc", "awm_device_free",
 ]
 
 _lib = None
@@ -136,6 +138,24 @@ def batch_keys_validate(items, n_values: int, key_index, n_keys: int, sample_rat
     err = ctypes.create_string_buffer(256)
     rc = load().awm_batch_keys_validate(_ptr(it), ctypes.c_size_t(len(it)), ctypes.c_size_t(n_values), _ptr(rates), _ptr(emit), _ptr(zf), _ptr(ki),
                                         ctypes.c_size_t(n_keys), ctypes.c_int(mark_sample_rate), err, ctypes.c_size_t(len(err)))
+    return err.value.decode() if rc else ""
+
+
+def resample_taps(n_in_total: int, ratio: float, out_first: int, out_frames: int, hlen: int = 16) -> tuple[int, int]:
+    """awm_resample_taps: input frames [first, end) the taps of outputs [out_first, out_first + out_frames) read, inside the stream"""
+    first, end = ctypes.c_uint64(), ctypes.c_uint64()
+    load().awm_resample_taps(ctypes.c_uint64(n_in_total), ctypes.c_double(ratio), ctypes.c_int(hlen), ctypes.c_uint64(out_first),
+                             ctypes.c_uint64(out_frames), ctypes.byref(first), ctypes.byref(end))
+    return first.value, end.value
+
+
+def resample_range_validate(in_first: int, in_frames: int, n_in_total: int, channels: int, ratio: float, out_first: int, out_frames: int,
+                            hlen: int = 16) -> str:
+    """awm_resample_range_validate: '' if awm_resample_range accepts the window, the ratio and the output range, else the reason"""
+    err = ctypes.create_string_buffer(256)
+    rc = load().awm_resample_range_validate(ctypes.c_uint64(in_first), ctypes.c_uint64(in_frames), ctypes.c_uint64(n_in_total), ctypes.c_int(channels),
+                                            ctypes.c_double(ratio), ctypes.c_int(hlen), ctypes.c_uint64(out_first), ctypes.c_uint64(out_frames), err,
+                                            ctypes.c_size_t(len(err)))
     return err.value.decode() if rc else ""
 
 
@@ -397,6 +417,18 @@ class Context:
         self._ck(self.lib.awm_resample(self.h, _ptr(pcm), ctypes.c_size_t(n_frames), ctypes.c_int(channels), ctypes.c_double(ratio), ctypes.c_int(hlen),
                                        _ptr(res), ctypes.c_size_t(n_out)))
         return res
+
+    def resample_range(self, window, in_first: int, n_in_total: int, ratio: float, out, out_first: int, out_frames: int, hlen: int = 16,
+                       in_frames=None, channels=None):
+        """awm_resample_range: outputs [out_first, out_first + out_frames) of resampling a stream of n_in_total frames, read from the
+        window of stream frames [in_first, in_first + in_frames) (numpy [n, ch], or a device pointer with in_frames / channels given),
+        written to the device pointer out"""
+        if isinstance(window, np.ndarray):
+            window = np.ascontiguousarray(window, np.float32)
+            in_frames, channels = window.shape
+        self._ck(self.lib.awm_resample_range(self.h, _ptr(window), ctypes.c_uint64(in_first), ctypes.c_uint64(in_frames), ctypes.c_uint64(n_in_total),
+                                             ctypes.c_int(channels), ctypes.c_double(ratio), ctypes.c_int(hlen), _ptr(out), ctypes.c_uint64(out_first),
+                                             ctypes.c_uint64(out_frames)))
 
     def pcm_push_resampled(self, ratio: float, n_out: int, hlen: int = 16):
         self._ck(self.lib.awm_pcm_push_resampled(self.h, ctypes.c_double(ratio), ctypes.c_int(hlen), ctypes.c_size_t(n_out)))

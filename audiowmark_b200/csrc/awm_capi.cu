@@ -2663,6 +2663,141 @@ awm_resample (awm_ctx *ctx, const float *in, size_t n_in, int channels, double r
   return 0;
 }
 
+uint64_t
+awm_resample_stream_available (uint64_t fed, double ratio, int hlen)
+{
+  const double fc = ratio < 1 ? ratio : 1;
+  const int h = int (ceil (hlen / fc));
+  const double step = 1.0 / ratio;
+  if ((long long) fed - 2 < h - 1)
+    return 0;
+  const double limit = double (fed) - 2;            /* centre tap (in pre-roll coordinates) of the last output that fits */
+  long long n = (long long) ((double (fed) - 1 - h) * ratio) - 2;
+  if (n < 0)
+    n = 0;
+  while (n > 0 && floor ((h - 1) + double (n - 1) * step) > limit)
+    n--;
+  while (floor ((h - 1) + double (n) * step) <= limit)
+    n++;
+  return uint64_t (n);
+}
+
+uint64_t
+awm_resample_stream_frames (uint64_t n_in, double ratio, int hlen)
+{
+  const double fc = ratio < 1 ? ratio : 1;
+  return awm_resample_stream_available (n_in + uint64_t (ceil (hlen / fc)), ratio, hlen);
+}
+
+void
+awm_resample_taps (uint64_t n_in_total, double ratio, int hlen, uint64_t out_first, uint64_t out_frames, uint64_t *first, uint64_t *end)
+{
+  *first = *end = 0;
+  if (!out_frames)
+    return;
+  const double fc = ratio < 1 ? ratio : 1;
+  const long long h = (long long) ceil (hlen / fc);
+  const double step = 1.0 / ratio;
+  /* c (n) of resample_pos, rounded the same way: a product and a sum, not fused */
+  auto centre = [&] (uint64_t n) { volatile double p = double (n) * step; return (long long) floor (double (h - 1) + p); };
+  const long long lo = centre (out_first) - 2 * h + 2, hi = centre (out_first + out_frames - 1) + 2;
+  *first = uint64_t (std::min<long long> (std::max (lo, 0LL), (long long) n_in_total));
+  *end = uint64_t (std::min<long long> (std::max (hi, (long long) *first), (long long) n_in_total));
+}
+
+int
+awm_resample_range_validate (uint64_t in_first, uint64_t in_frames, uint64_t n_in_total, int channels, double ratio, int hlen,
+                             uint64_t out_first, uint64_t out_frames, char *err, size_t err_cap)
+{
+  char why[240] = "";
+  uint64_t t0 = 0, t1 = 0;
+  if (channels <= 0)
+    snprintf (why, sizeof (why), "channels %d must be > 0", channels);
+  else if (!resample_ratio_ok (ratio) || hlen < 8 || hlen > 96)
+    snprintf (why, sizeof (why), "ratio %g / hlen %d not supported (ratio in (1/64, 64), hlen in [8, 96])", ratio, hlen);
+  else if (n_in_total > AWM_MAX_STREAM_FRAMES || out_first > AWM_MAX_STREAM_FRAMES || out_frames > AWM_MAX_STREAM_FRAMES
+           || in_first > AWM_MAX_STREAM_FRAMES || in_frames > AWM_MAX_STREAM_FRAMES)
+    snprintf (why, sizeof (why), "frame counts and positions must be at most 2^48");
+  else if (out_first + out_frames > awm_resample_stream_frames (n_in_total, ratio, hlen))
+    snprintf (why, sizeof (why), "outputs [%llu, %llu) end past the %llu frames of the resampled stream", (unsigned long long) out_first,
+              (unsigned long long) (out_first + out_frames), (unsigned long long) awm_resample_stream_frames (n_in_total, ratio, hlen));
+  else
+    {
+      awm_resample_taps (n_in_total, ratio, hlen, out_first, out_frames, &t0, &t1);
+      if (t0 < t1 && (t0 < in_first || t1 > in_first + in_frames))
+        snprintf (why, sizeof (why), "outputs [%llu, %llu) read input frames [%llu, %llu), the window holds [%llu, %llu)", (unsigned long long) out_first,
+                  (unsigned long long) (out_first + out_frames), (unsigned long long) t0, (unsigned long long) t1, (unsigned long long) in_first,
+                  (unsigned long long) (in_first + in_frames));
+    }
+  if (err && err_cap)
+    snprintf (err, err_cap, "%s", why);
+  return why[0] ? 1 : 0;
+}
+
+int
+awm_resample_range (awm_ctx *ctx, const float *in, uint64_t in_first, uint64_t in_frames, uint64_t n_in_total, int channels, double ratio, int hlen,
+                    float *out, uint64_t out_first, uint64_t out_frames)
+{
+  char why[240];
+  if (awm_resample_range_validate (in_first, in_frames, n_in_total, channels, ratio, hlen, out_first, out_frames, why, sizeof (why)))
+    return fail (ctx, "awm_resample_range: %s", why);
+  if ((in_frames && !in) || (out_frames && !out))
+    return fail (ctx, "awm_resample_range: bad arguments");
+  if (!out_frames)
+    return 0;
+  CK (cudaSetDevice (ctx->device));
+  if (!is_device_ptr (out))
+    return fail (ctx, "awm_resample_range: out must be device memory");
+  const float *coef;
+  int h;
+  if (coef_table (ctx, ratio, hlen, &coef, &h))
+    return 1;
+  ResampleJob J;
+  J.in = in;
+  J.out = out;
+  if (in_frames && !is_device_ptr (in))
+    {
+      CK (ctx->rs_in.reserve (in_frames * channels * sizeof (float)));
+      CK (cudaMemcpyAsync (ctx->rs_in.p, in, in_frames * channels * sizeof (float), cudaMemcpyHostToDevice, ctx->stream));
+      J.in = ctx->rs_in.as<float>();
+    }
+  J.n0 = (long long) out_first;
+  J.in0 = (long long) in_first;
+  J.n_in = (long long) n_in_total - J.in0;               /* the window-relative tap test i < n_in is the stream's i < n_in_total */
+  J.n_stop = (long long) n_in_total;
+  J.n_out = (long long) out_frames;
+  J.step = 1.0 / ratio;
+  J.h = h;
+  J.coef = coef;
+  return launch_resample (ctx, { J }, channels);
+}
+
+int
+awm_device_alloc (awm_ctx *ctx, size_t bytes, void **out)
+{
+  if (!ctx || !out)
+    return fail (ctx, "awm_device_alloc: bad arguments");
+  *out = nullptr;
+  if (!bytes)
+    return 0;
+  CK (cudaSetDevice (ctx->device));
+  CK (cudaMalloc (out, bytes));
+  return 0;
+}
+
+int
+awm_device_free (awm_ctx *ctx, void *p)
+{
+  if (!ctx)
+    return 1;
+  if (!p)
+    return 0;
+  CK (cudaSetDevice (ctx->device));
+  CK (cudaStreamSynchronize (ctx->stream));              /* kernels queued on the context stream may still read it */
+  CK (cudaFree (p));
+  return 0;
+}
+
 int
 awm_pcm_push_resampled (awm_ctx *ctx, double ratio, int hlen, size_t n_out)
 {

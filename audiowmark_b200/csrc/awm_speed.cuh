@@ -27,6 +27,9 @@ struct ResampleJob
   int          h;           // half filter length in input frames; 2h taps
   const float *coef;        // [2h][kResamplePhases + 1]: tap major, so that the lanes of a warp (same tap, different phase)
                             // gather inside one 1 KB row instead of touching 32 different rows
+  // a range of a longer stream (awm_resample_range): out[n] is output n0 + n of the stream, in[i] is stream frame in0 + i, and
+  // n_in / n_stop count from in0 / from 0; both 0 for a whole stream
+  long long    n0 = 0, in0 = 0;
 };
 
 // out[n] = sum_j x[c - 2h + 2 + j] * ((1-a) coef[p][j] + a coef[p+1][j]),  t = (h-1) + n step, c = floor t,
@@ -105,12 +108,13 @@ k_resample (const ResampleJob *__restrict__ jobs, int c_dyn)
     {
       float *o = J.out + n * CH;
       ResamplePos P;
-      if (!resample_pos (J, n, P))
+      if (!resample_pos (J, J.n0 + n, P))
         {
           for (int ch = 0; ch < CH; ch++)
             o[ch] = 0.0f;
           continue;
         }
+      P.i0 -= J.in0;                                          // stream frame -> frame of the input window
       if (C == 2)
         reinterpret_cast<float2 *> (J.out)[n] = resample_dot2 (J, P);
       else

@@ -1,6 +1,7 @@
 // awm_balanced.cc -- see awm_balanced.hh
 #include "awm_balanced.hh"
 #include "awm_engine.hh"
+#include "awm_speed.hh"
 #include "awm_tables.hh"
 #include "awm_util.hh"
 
@@ -163,6 +164,46 @@ owner_of (const vector<Chunk>& plan, size_t n_total, int world, int chunk, uint6
   return int (std::min<size_t> (pos / owner_span (n_total, world), world - 1));
 }
 
+bool
+rate_supported (int sample_rate)
+{
+  if (sample_rate <= 0)
+    return false;
+  const double up = double (Params::mark_sample_rate) / sample_rate, down = double (sample_rate) / Params::mark_sample_rate;
+  return up > 1.0 / 64 && up < 64 && down > 1.0 / 64 && down < 64;
+}
+
+size_t
+mark_frames (size_t n_total, int sample_rate)
+{
+  return sample_rate == Params::mark_sample_rate ? n_total : resample_stream_frames (n_total, double (Params::mark_sample_rate) / sample_rate);
+}
+
+void
+input_range (const vector<Slice>& slices, size_t n_total, int sample_rate, size_t& first, size_t& end)
+{
+  first = end = 0;
+  if (slices.empty())
+    return;
+  size_t lo = slices[0].lo, hi = slices[0].hi;
+  for (const Slice& sl : slices)
+    {
+      lo = std::min (lo, sl.lo);
+      hi = std::max (hi, sl.hi);
+    }
+  if (sample_rate == Params::mark_sample_rate)
+    {
+      first = lo;
+      end = hi;
+      return;
+    }
+  uint64_t t0, t1;
+  awm_resample_taps (n_total, double (Params::mark_sample_rate) / sample_rate, 16, lo, hi - lo, &t0, &t1);
+  /* one frame on each side: the range stays whole even if a build evaluates the tap positions with a fused multiply-add */
+  first = t0 ? size_t (t0) - 1 : 0;
+  end = std::min<size_t> (size_t (t1) + 1, n_total);
+}
+
 /* ---------------------------------------------------------------------------------------------------------------- Get */
 
 Get::Get (int rank, int world, size_t n_total, const float *pcm, const int16_t *pcm16, size_t pcm_start, size_t pcm_frames, int channels,
@@ -170,32 +211,71 @@ Get::Get (int rank, int world, size_t n_total, const float *pcm, const int16_t *
   m_rank (rank), m_world (world), m_channels (channels), m_rate (sample_rate), m_n_total (n_total), m_pcm_start (pcm_start), m_pcm_frames (pcm_frames), m_key (key)
 {
   awm_ctx *ctx = Engine::ctx();
-  if (!ctx || sample_rate != Params::mark_sample_rate || (!pcm && !pcm16))
+  if (!ctx || !rate_supported (sample_rate) || (!pcm && !pcm16))
     {
-      error ("audiowmark: sharded get needs a CUDA device and input at %d Hz\n", Params::mark_sample_rate);
+      error ("audiowmark: sharded get needs a CUDA device and input at a sample rate of %d Hz / 64 .. %d Hz * 64 (exclusive), not %d Hz\n",
+             Params::mark_sample_rate, Params::mark_sample_rate, sample_rate);
       return;
     }
   m_slot = Engine::key_slot (key);
   if (m_slot < 0)
     return;
+  const bool resampled = sample_rate != Params::mark_sample_rate;
+  const double ratio = double (Params::mark_sample_rate) / sample_rate;
+  m_n_mark = mark_frames (n_total, sample_rate);
   /* inputs short enough for the reference's ClipDecoder (src/wmget.cc:764-884: fewer than 3.1 blocks) are a few seconds of work on one
    * GPU; the sharded driver only runs the block decoder, so it refuses them instead of returning a document without CLIP patterns */
-  if (double (n_total / Params::frame_size) < double (frames_per_block()) * 3.1)
+  if (double (m_n_mark / Params::frame_size) < double (frames_per_block()) * 3.1)
     {
-      error ("audiowmark: sharded get: input of %zu frames is clip sized (under 3.1 blocks); use the single GPU get\n", n_total);
+      error ("audiowmark: sharded get: input of %zu frames (%zu at %d Hz) is clip sized (under 3.1 blocks); use the single GPU get\n", n_total,
+             m_n_mark, Params::mark_sample_rate);
       return;
     }
-  m_plan = chunk_plan (n_total, sample_rate);
-  m_slices = rank_slices (m_plan, rank, world, n_total);
+  m_plan = chunk_plan (m_n_mark, Params::mark_sample_rate);
+  m_slices = rank_slices (m_plan, rank, world, m_n_mark);
   for (int r = 0; r < world; r++)                // which ranks search a slice of which chunk (ascending rank order)
-    for (const Slice& sl : rank_slices (m_plan, r, world, n_total))
+    for (const Slice& sl : rank_slices (m_plan, r, world, m_n_mark))
       m_sharers[sl.chunk].push_back (r);
-  for (const Slice& sl : m_slices)
-    if (sl.lo < pcm_start || sl.hi > pcm_start + pcm_frames)
-      {
-        error ("audiowmark: sharded get: rank %d needs stream frames [%zu, %zu), its buffer holds [%zu, %zu)\n", rank, sl.lo, sl.hi, pcm_start, pcm_start + pcm_frames);
-        return;
-      }
+  if (!resampled)
+    {
+      for (const Slice& sl : m_slices)
+        if (sl.lo < pcm_start || sl.hi > pcm_start + pcm_frames)
+          {
+            error ("audiowmark: sharded get: rank %d needs stream frames [%zu, %zu), its buffer holds [%zu, %zu)\n", rank, sl.lo, sl.hi, pcm_start, pcm_start + pcm_frames);
+            return;
+          }
+    }
+  else if (!m_slices.empty())
+    {
+      size_t first, end;
+      input_range (m_slices, n_total, sample_rate, first, end);
+      if (first < pcm_start || end > pcm_start + pcm_frames)
+        {
+          error ("audiowmark: sharded get: rank %d needs stream frames [%zu, %zu) at %d Hz, its buffer holds [%zu, %zu)\n", rank, first, end, sample_rate,
+                 pcm_start, pcm_start + pcm_frames);
+          return;
+        }
+      size_t lo = m_slices[0].lo, hi = m_slices[0].hi;        // chunks overlap: a later slice can begin before an earlier one
+      for (const Slice& sl : m_slices)
+        {
+          lo = std::min (lo, sl.lo);
+          hi = std::max (hi, sl.hi);
+        }
+      m_mark_lo = m_mark_done = lo;
+      char why[240];
+      if (awm_resample_range_validate (pcm_start, pcm_frames, n_total, channels, ratio, 16, m_mark_lo, hi - m_mark_lo, why, sizeof (why)))
+        {
+          error ("audiowmark: sharded get: %s\n", why);
+          return;
+        }
+      void *buf = nullptr;
+      if (awm_device_alloc (ctx, (hi - m_mark_lo) * channels * sizeof (float), &buf))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return;
+        }
+      m_mark = static_cast<float *> (buf);
+    }
   /* one upload for all stages, piece by piece: the stages bind slices of the device copy, a slice waits only for the pieces it reads */
   if (pcm && Engine::is_device_pointer (pcm))
     m_dev = pcm;
@@ -212,6 +292,12 @@ Get::Get (int rank, int world, size_t n_total, const float *pcm, const int16_t *
   m_ok = true;
 }
 
+Get::~Get()
+{
+  if (m_mark)
+    awm_device_free (Engine::ctx(), m_mark);
+}
+
 const Slice *
 Get::my_slice (int chunk) const
 {
@@ -225,8 +311,33 @@ bool
 Get::bind (const Slice& sl)
 {
   awm_ctx *ctx = Engine::ctx();
-  if ((m_staged && awm_pcm_stage_wait (ctx, sl.hi - m_pcm_start))
-      || awm_pcm_bind (ctx, m_dev + (sl.lo - m_pcm_start) * m_channels, sl.hi - sl.lo, m_channels, 0, 0))
+  if (!m_mark)
+    {
+      if ((m_staged && awm_pcm_stage_wait (ctx, sl.hi - m_pcm_start))
+          || awm_pcm_bind (ctx, m_dev + (sl.lo - m_pcm_start) * m_channels, sl.hi - sl.lo, m_channels, 0, 0))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return false;
+        }
+      return true;
+    }
+  /* [m_mark_lo, m_mark_done) is resampled: compute only the outputs no earlier bind produced, after the input pieces their taps
+   * read have arrived */
+  if (sl.hi > m_mark_done)
+    {
+      const double ratio = double (Params::mark_sample_rate) / m_rate;
+      uint64_t t0, t1;
+      awm_resample_taps (m_n_total, ratio, 16, m_mark_done, sl.hi - m_mark_done, &t0, &t1);
+      if ((m_staged && awm_pcm_stage_wait (ctx, std::max<size_t> (t1, m_pcm_start) - m_pcm_start))
+          || awm_resample_range (ctx, m_dev, m_pcm_start, m_pcm_frames, m_n_total, m_channels, ratio, 16, m_mark + (m_mark_done - m_mark_lo) * m_channels,
+                                 m_mark_done, sl.hi - m_mark_done))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return false;
+        }
+      m_mark_done = sl.hi;
+    }
+  if (awm_pcm_bind (ctx, m_mark + (sl.lo - m_mark_lo) * m_channels, sl.hi - sl.lo, m_channels, 0, 0))
     {
       error ("audiowmark: %s\n", awm_last_error (ctx));
       return false;
@@ -374,7 +485,7 @@ Get::stage_refine_decode (string& out)
       vector<uint32_t> mine;
       vector<awm_search_score> part;
       for (size_t i = 0; i < kv.second.size(); i++)
-        if (owner_of (m_plan, m_n_total, m_world, chunk, kv.second[i].index) == m_rank)
+        if (owner_of (m_plan, m_n_mark, m_world, chunk, kv.second[i].index) == m_rank)
           {
             mine.push_back (uint32_t (i));
             part.push_back (kv.second[i]);
@@ -495,7 +606,7 @@ Get::stage_viterbi (const vector<string>& all, string& out)
               }
           }
       vector<VitJob> chunk_jobs;
-      build_block_jobs (m_key, final_scores, soft, valid, m_rate, kv.first, 1.0, chunk_jobs);
+      build_block_jobs (m_key, final_scores, soft, valid, Params::mark_sample_rate, kv.first, 1.0, chunk_jobs);
       const vector<int>& sharers = m_sharers[kv.first];
       for (size_t j = 0; j < chunk_jobs.size(); j++)
         if (sharers[j % sharers.size()] == m_rank)

@@ -38,17 +38,32 @@ std::vector<Slice> rank_slices (const std::vector<Chunk>& plan, int rank, int wo
 /* rank that owns a chunk-relative sample index (by the start frame it falls into) */
 int owner_of (const std::vector<Chunk>& plan, size_t n_total, int world, int chunk, uint64_t index);
 
+/* Input at another sample rate: the single GPU get resamples the stream to the watermark rate first and plans there, and so does
+ * the sharded get -- chunk_plan, rank_slices and owner_of above all take the watermark-rate stream of mark_frames (n_total) frames. */
+bool rate_supported (int sample_rate);       /* both resampling ratios inside the resampler's range (1/64, 64) */
+size_t mark_frames (size_t n_total, int sample_rate);
+/* input frames [first, end) of a stream of n_total frames at sample_rate that a rank with these slices reads: at the watermark
+ * rate the union [min lo, max hi) of its slices, at other rates every frame the resampler taps of that union read, plus one frame
+ * on each side, inside [0, n_total); [0, 0) without slices */
+void input_range (const std::vector<Slice>& slices, size_t n_total, int sample_rate, size_t& first, size_t& end);
+
 /* every rank contributes one byte string and receives everybody's, in rank order */
 typedef std::function<bool (const std::string& mine, std::vector<std::string>& all)> Exchange;
 
 class Get
 {
 public:
-  /* pcm / pcm16: this rank's part of the stream (host or device memory; exactly one of the two), starting at stream frame
-   * pcm_start; it must cover every slice of the rank (rank_slices) */
+  /* pcm / pcm16: this rank's part of the stream of n_total frames at sample_rate (host or device memory; exactly one of the two),
+   * starting at stream frame pcm_start; it must cover input_range of the rank's slices.  At another rate than the watermark rate
+   * the rank resamples what its slices need into a buffer of its own as it binds them (host input is uploaded piece by piece, a
+   * slice waits only for the pieces its taps read) */
   Get (int rank, int world, size_t n_total, const float *pcm, const int16_t *pcm16, size_t pcm_start, size_t pcm_frames, int channels,
        int sample_rate, const Key& key);
+  ~Get();
+  Get (const Get&) = delete;
+  Get& operator= (const Get&) = delete;
   bool ok() const { return m_ok; }
+  size_t n_mark() const { return m_n_mark; }      /* frames of the stream at the watermark rate */
 
   /* the stages, callable one by one (tests drive several ranks in one process) */
   bool stage_peaks (const std::map<int, double>& floors, std::string& out);
@@ -65,8 +80,10 @@ private:
   const Slice *my_slice (int chunk) const;
 
   int    m_rank, m_world, m_channels, m_rate, m_slot = -1;
-  size_t m_n_total, m_pcm_start, m_pcm_frames;
+  size_t m_n_total, m_n_mark = 0, m_pcm_start, m_pcm_frames;
   const float *m_dev = nullptr;    // device copy of this rank's PCM
+  float *m_mark = nullptr;         // other rates: watermark-rate frames [m_mark_lo, max hi of the slices) of the stream
+  size_t m_mark_lo = 0, m_mark_done = 0;    // ... of which [m_mark_lo, m_mark_done) are resampled
   Key    m_key;
   bool   m_ok = false, m_staged = false;
   std::vector<Chunk> m_plan;

@@ -740,11 +740,12 @@ awmh_balanced_get (const unsigned char *key16, const void *pcm, int is_s16, uint
         *n_patterns = -1;
       return 0;
     }
-  return result_json (result_set, n_total, json_out, json_cap, n_patterns);
+  return result_json (result_set, job.n_mark(), json_out, json_cap, n_patterns);
 }
 
 /* the stages one by one, for tests that run several ranks in one process on one GPU (tests/test_gpu_sharding.py):
- * stage 0 peaks, 1 select (-> retry list), 2 peaks again for the retry list in in[0], 3 refine + soft bits, 4 viterbi, 5 merge (-> JSON) */
+ * stage 0 peaks, 1 select (-> retry list), 2 peaks again for the retry list in in[0], 3 refine + soft bits, 4 viterbi, 5 merge (-> JSON;
+ * its length is that of the watermark-rate stream the driver planned, awmh_bg_stage's n_total is not used) */
 void *
 awmh_bg_create (const unsigned char *key16, int rank, int world, const float *pcm, uint64_t pcm_start, uint64_t pcm_frames, uint64_t n_total, int n_channels, int sample_rate)
 {
@@ -810,7 +811,7 @@ awmh_bg_stage (void *h, int stage, const unsigned char *const *in, const size_t 
             char *buf = nullptr;
             size_t len = 0;
             FILE *f = open_memstream (&buf, &len);
-            rs.print_json (f, size_t (lrint (double (n_total) / Params::mark_sample_rate)));
+            rs.print_json (f, size_t (lrint (double (g->n_mark()) / Params::mark_sample_rate)));
             fclose (f);
             res.assign (buf, len);
             free (buf);
@@ -828,12 +829,17 @@ awmh_bg_stage (void *h, int stage, const unsigned char *const *in, const size_t 
   return 0;
 }
 
-/* the plan functions for CPU tests: chunk walk, slices of a rank, owner of an index */
+/* the plan functions for CPU tests and launchers: chunk walk, slices of a rank, owner of an index, the input a rank holds.  A stream of
+ * n_total frames at sample_rate is planned at the watermark rate, as the driver runs it (balanced::mark_frames); 1 for a sample rate
+ * the sharded get refuses */
 int
 awmh_bg_plan (uint64_t n_total, int sample_rate, int rank, int world, double *chunks /* [max][3] first, count, time offset */, int max_chunks, int *n_chunks,
               int64_t *slices /* [max][7] chunk, sa, sb, a, b, lo, hi */, int max_slices, int *n_slices)
 {
-  const auto plan = balanced::chunk_plan (n_total, sample_rate);
+  if (!balanced::rate_supported (sample_rate))
+    return 1;
+  const size_t n_mark = balanced::mark_frames (n_total, sample_rate);
+  const auto plan = balanced::chunk_plan (n_mark, Params::mark_sample_rate);
   *n_chunks = int (plan.size());
   for (int c = 0; c < int (plan.size()) && c < max_chunks; c++)
     {
@@ -841,7 +847,7 @@ awmh_bg_plan (uint64_t n_total, int sample_rate, int rank, int world, double *ch
       chunks[3 * c + 1] = double (plan[c].count);
       chunks[3 * c + 2] = plan[c].time_offset;
     }
-  const auto sl = balanced::rank_slices (plan, rank, world, n_total);
+  const auto sl = balanced::rank_slices (plan, rank, world, n_mark);
   *n_slices = int (sl.size());
   for (int i = 0; i < int (sl.size()) && i < max_slices; i++)
     {
@@ -854,7 +860,24 @@ awmh_bg_plan (uint64_t n_total, int sample_rate, int rank, int world, double *ch
 int
 awmh_bg_owner (uint64_t n_total, int sample_rate, int world, int chunk, uint64_t index)
 {
-  return balanced::owner_of (balanced::chunk_plan (n_total, sample_rate), n_total, world, chunk, index);
+  if (!balanced::rate_supported (sample_rate))
+    return -1;
+  const size_t n_mark = balanced::mark_frames (n_total, sample_rate);
+  return balanced::owner_of (balanced::chunk_plan (n_mark, Params::mark_sample_rate), n_mark, world, chunk, index);
+}
+
+/* input frames [*first, *end) of the stream that rank `rank` of `world` has to hold (balanced::input_range of its slices) */
+int
+awmh_bg_input_range (uint64_t n_total, int rank, int world, int sample_rate, uint64_t *first, uint64_t *end)
+{
+  if (!balanced::rate_supported (sample_rate) || world < 1 || rank < 0 || rank >= world)
+    return 1;
+  const size_t n_mark = balanced::mark_frames (n_total, sample_rate);
+  size_t f, e;
+  balanced::input_range (balanced::rank_slices (balanced::chunk_plan (n_mark, Params::mark_sample_rate), rank, world, n_mark), n_total, sample_rate, f, e);
+  *first = f;
+  *end = e;
+  return 0;
 }
 
 /* ---- stage-level access for the frame-balanced multi-GPU driver (audiowmark_b200/sharding.py) ---------------- */

@@ -375,28 +375,12 @@ resample_ratio (const float *in, size_t n_frames, int n_channels, double ratio, 
 size_t
 resample_stream_available (size_t fed, double ratio)
 {
-  const int hlen = 16;
-  const double fc = ratio < 1 ? ratio : 1;
-  const int h = int (ceil (hlen / fc));
-  const double step = 1.0 / ratio;
-  if ((long long) fed - 2 < h - 1)
-    return 0;
-  const double limit = double (fed) - 2;            /* centre tap (in pre-roll coordinates) of the last output that fits */
-  long long n = (long long) ((double (fed) - 1 - h) * ratio) - 2;
-  if (n < 0)
-    n = 0;
-  while (n > 0 && floor ((h - 1) + double (n - 1) * step) > limit)
-    n--;
-  while (floor ((h - 1) + double (n) * step) <= limit)
-    n++;
-  return size_t (n);
+  return awm_resample_stream_available (fed, ratio, 16);
 }
 
 /* ... plus write_trailing_frames (k/2 zero frames, src/resample.cc:198-204): what WavChunkLoader gets for n_in input frames */
 size_t
 resample_stream_frames (size_t n_in, double ratio)
 {
-  const double fc = ratio < 1 ? ratio : 1;
-  const int h = int (ceil (16 / fc));
-  return resample_stream_available (n_in + h, ratio);
+  return awm_resample_stream_frames (n_in, ratio, 16);
 }

@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libawm_host.so")
 CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
-           "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_add_windowed",
+           "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_bg_input_range", "awmh_add_windowed",
            "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16", "awmh_add_batch_rates", "awmh_add_batch_rates_s16",
            "awmh_add_batch_offsets", "awmh_add_batch_offsets_s16", "awmh_add_batch_rates_offsets", "awmh_add_batch_rates_offsets_s16",
            "awmh_add_batch_keys", "awmh_add_batch_keys_s16", "awmh_role_layout", "awmh_embed_roles_device"]
@@ -582,7 +582,9 @@ def dist_init_from_torch():
 
 def balanced_get(pcm, pcm_start: int, n_total: int, key=None, n_frames=None, channels=None, sample_rate=44100, parse=True):
     """this rank's part of the stream (numpy float32 / int16 [n, ch], or a float32 device pointer) -> the --json document on rank 0
-    (parse=False: its text, as `audiowmark get --json` writes it), None on the other ranks"""
+    (parse=False: its text, as `audiowmark get --json` writes it), None on the other ranks.  The part starts at stream frame
+    pcm_start and must cover balanced_input_range(n_total, rank, world, sample_rate); at a rate other than 44.1 kHz every rank
+    resamples only that part, on its device"""
     is_s16 = 0
     if isinstance(pcm, np.ndarray):
         if pcm.dtype == np.int16:
@@ -609,7 +611,7 @@ class BalancedStages:
     def __init__(self, rank, world, n_total, pcm_device_ptr: int, pcm_frames: int, channels: int, pcm_start, key=None, sample_rate=44100):
         """pcm_device_ptr: float32 [pcm_frames, channels] in device memory that stays valid while the object lives (several ranks in
         one process share the context, so each needs its own device copy -- a host buffer would land in the context's single
-        upload buffer)"""
+        upload buffer); stream frames [pcm_start, pcm_start + pcm_frames) at sample_rate, covering balanced_input_range"""
         self.n_total = n_total
         L = load()
         L.awmh_bg_create.restype = ctypes.c_void_p
@@ -638,17 +640,33 @@ class BalancedStages:
 
 
 def balanced_plan(n_total: int, rank: int, world: int, sample_rate=44100):
-    """-> (chunks [(first, count, time offset)], slices [(chunk, sa, sb, a, b, lo, hi)]) as the C++ driver computes them"""
+    """-> (chunks [(first, count, time offset)], slices [(chunk, sa, sb, a, b, lo, hi)]) as the C++ driver computes them.  A stream of
+    n_total frames at sample_rate is planned as the driver runs it: in 44.1 kHz frames of the stream resampled to the watermark rate"""
     chunks = np.zeros((64, 3), np.float64)
     slices = np.zeros((64, 7), np.int64)
     nc, ns = ctypes.c_int(), ctypes.c_int()
-    load().awmh_bg_plan(ctypes.c_uint64(n_total), ctypes.c_int(sample_rate), ctypes.c_int(rank), ctypes.c_int(world), _ptr(chunks), ctypes.c_int(64), ctypes.byref(nc),
-                        _ptr(slices), ctypes.c_int(64), ctypes.byref(ns))
+    if load().awmh_bg_plan(ctypes.c_uint64(n_total), ctypes.c_int(sample_rate), ctypes.c_int(rank), ctypes.c_int(world), _ptr(chunks), ctypes.c_int(64),
+                           ctypes.byref(nc), _ptr(slices), ctypes.c_int(64), ctypes.byref(ns)):
+        raise ValueError("sharded get: sample rate %d Hz is outside the resampler's range" % sample_rate)
     return [(int(a), int(b), float(t)) for a, b, t in chunks[:nc.value]], [tuple(int(v) for v in row) for row in slices[:ns.value]]
 
 
 def balanced_owner(n_total: int, world: int, chunk: int, index: int, sample_rate=44100) -> int:
-    return load().awmh_bg_owner(ctypes.c_uint64(n_total), ctypes.c_int(sample_rate), ctypes.c_int(world), ctypes.c_int(chunk), ctypes.c_uint64(index))
+    r = load().awmh_bg_owner(ctypes.c_uint64(n_total), ctypes.c_int(sample_rate), ctypes.c_int(world), ctypes.c_int(chunk), ctypes.c_uint64(index))
+    if r < 0:
+        raise ValueError("sharded get: sample rate %d Hz is outside the resampler's range" % sample_rate)
+    return r
+
+
+def balanced_input_range(n_total: int, rank: int, world: int, sample_rate=44100) -> tuple[int, int]:
+    """stream frames [first, end) at sample_rate that rank `rank` of `world` has to hold for balanced_get: the union of its slices at
+    44.1 kHz; at other rates every frame the resampler taps of that union read, plus one frame on each side.  (0, 0) for a rank
+    without slices"""
+    first, end = ctypes.c_uint64(), ctypes.c_uint64()
+    if load().awmh_bg_input_range(ctypes.c_uint64(n_total), ctypes.c_int(rank), ctypes.c_int(world), ctypes.c_int(sample_rate), ctypes.byref(first),
+                                  ctypes.byref(end)):
+        raise ValueError("sharded get: sample rate %d Hz / rank %d of %d not supported" % (sample_rate, rank, world))
+    return first.value, end.value
 
 
 def engine_ctx() -> int:

@@ -124,8 +124,11 @@ def gather_blobs(blobs, device=None):
 # decide which part of the stream a rank has to hold (and embed), tests/test_sharding_cpu.py checks that both agree.
 # =====================================================================================================================
 
+import math
+
 import numpy as np
 
+MARK_RATE = 44100              # the watermark rate: a stream at another rate is planned after resampling to it
 T_BLOCK = 2226                 # frames per block (payload 128 bit): sync pattern length in BLOCK mode
 MARGIN = 6                     # start frames of margin on each side of a slice (local mean uses +-20 scores = +-5 frames)
 
@@ -171,3 +174,24 @@ def index_owners(plan, n_total: int, world: int, chunk: int, indices) -> np.ndar
     s = np.clip(np.asarray(indices, np.int64) // FRAME, 0, max(n_starts - 1, 0))
     span = owner_span(n_total, world)
     return np.minimum((cs + s * FRAME) // span, world - 1)
+
+
+def rank_input_range(slices, n_total: int, sample_rate: int):
+    """stream frames [first, end) at sample_rate that a rank with these slices (rank_slices of the stream at the watermark rate, of
+    hostapi.resample_stream_frames(n_total, 44100 / sample_rate) frames) has to hold: at 44.1 kHz the union [min lo, max hi) of its
+    slices; at other rates every input frame a resampler tap of that union reads -- output n has taps c(n) - 2h + 2 .. c(n) + 1,
+    c(n) = floor((h - 1) + n * step) -- plus one frame on each side, inside [0, n_total).  (0, 0) without slices."""
+    if not slices:
+        return 0, 0
+    lo, hi = min(sl.lo for sl in slices), max(sl.hi for sl in slices)
+    if sample_rate == MARK_RATE:
+        return lo, hi
+    ratio = MARK_RATE / sample_rate
+    h = int(math.ceil(16 / min(ratio, 1.0)))
+    step = 1.0 / ratio
+
+    def c(n):
+        return math.floor(float(h - 1) + float(n) * step)
+    first = min(max(c(lo) - 2 * h + 2 - 1, 0), n_total)
+    end = min(max(c(hi - 1) + 2 + 1, first), n_total)
+    return first, end

@@ -374,6 +374,28 @@ int awm_viterbi (awm_ctx *ctx, const float *raw_bits, size_t n_jobs, int n_msg_b
  */
 int awm_resample (awm_ctx *ctx, const float *in, size_t n_in, int channels, double ratio, int hlen, float *out, size_t n_out);
 
+/* Frames a streaming resampler (the reference's BufferedResamplerImpl) has delivered after `fed` input frames (pre-roll excluded),
+ * and after n_in frames plus its trailing frames: the length of the resampled stream.  hlen = 16 in the reference.  Needs no device. */
+uint64_t awm_resample_stream_available (uint64_t fed, double ratio, int hlen);
+uint64_t awm_resample_stream_frames (uint64_t n_in, double ratio, int hlen);
+/* Input frames [*first, *end) of a stream of n_in_total frames that the taps of outputs [out_first, out_first + out_frames) of
+ * awm_resample read, clamped to the stream (taps outside it read zero).  Needs no device. */
+void awm_resample_taps (uint64_t n_in_total, double ratio, int hlen, uint64_t out_first, uint64_t out_frames, uint64_t *first, uint64_t *end);
+/* Outputs [out_first, out_first + out_frames) of awm_resample over a whole stream of n_in_total frames, bit for bit, read from a
+ * window of that stream: in holds stream frames [in_first, in_first + in_frames) (interleaved float, host or device); out is a
+ * device buffer of out_frames frames.  Taps outside [0, n_in_total) read zero and outputs awm_resample zeroes (past its post-roll)
+ * are zero, as in awm_resample.  Refused before any work (awm_resample_range_validate, which needs no device): channels <= 0, a
+ * ratio outside (1/64, 64) or hlen outside [8, 96], counts or positions above 2^48, outputs that end past
+ * awm_resample_stream_frames (n_in_total, ratio, hlen), and a window that misses a frame awm_resample_taps names. */
+int awm_resample_range_validate (uint64_t in_first, uint64_t in_frames, uint64_t n_in_total, int channels, double ratio, int hlen,
+                                 uint64_t out_first, uint64_t out_frames, char *err, size_t err_cap);
+int awm_resample_range (awm_ctx *ctx, const float *in, uint64_t in_first, uint64_t in_frames, uint64_t n_in_total, int channels, double ratio, int hlen,
+                        float *out, uint64_t out_first, uint64_t out_frames);
+/* device memory on the context's device for callers without a device allocator of their own (bytes = 0: *out = NULL);
+ * awm_device_free waits for the work queued on the context stream before it frees */
+int awm_device_alloc (awm_ctx *ctx, size_t bytes, void **out);
+int awm_device_free (awm_ctx *ctx, void *p);
+
 /* resample_ratio (wav_data, speed, ...) of decode() (src/wmget.cc:916) without leaving the device: the bound PCM is
  * resampled by `ratio` into a context-owned buffer of n_out frames, which becomes the bound PCM; awm_pcm_pop restores
  * the previous binding (the original chunk is not copied again).  One level only; awm_pcm_bind drops a pushed binding. */
