@@ -114,8 +114,8 @@ add_watermark_buffer (const Key& key, const float *in, float *out, size_t n_fram
       /* a batch of one item: the embed at other rates exists in batched form only */
       const awm_batch_item item = { 0, n_frames, n_channels };
       vector<AddStats> item_stats;
-      if (add_watermark_batch_rates (key, in, out, false, n_frames * size_t (n_channels), &item, 1, { bits }, &sample_rate, 0,
-                                     stats ? &item_stats : nullptr))
+      if (add_watermark_batch ({ key }, false, in, out, false, n_frames * size_t (n_channels), &item, 1, { bits }, sample_rate, &sample_rate,
+                               nullptr, 0, stats ? &item_stats : nullptr))
         return 1;
       if (stats)
         *stats = item_stats[0];
@@ -168,142 +168,21 @@ add_watermark_buffer_s16 (const Key& key, const int16_t *in, int16_t *out, size_
 }
 
 int
-add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                     const vector<string>& bits, int sample_rate, vector<AddStats> *stats, const uint64_t *zero_frames)
+add_watermark_batch (const vector<Key>& keys, bool per_item_keys, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items,
+                     size_t n_items, const vector<string>& bits, int sample_rate, const int *sample_rates, const uint64_t *zero_frames,
+                     size_t scratch_bytes, vector<AddStats> *stats)
 {
-  char why[256];
-  if (zero_frames && awm_batch_offsets_validate (items, n_items, n_values, zero_frames, sample_rate, Params::mark_sample_rate, why, sizeof (why)))
-    {
-      error ("audiowmark: %s\n", why);
-      return 2;
-    }
-  if (sample_rate != Params::mark_sample_rate)
-    {
-      error ("audiowmark: batched embedding is only available at %d Hz\n", Params::mark_sample_rate);
-      return 2;
-    }
-  if (awm_batch_validate (items, n_items, n_values, why, sizeof (why)))
-    {
-      error ("audiowmark: %s\n", why);
-      return 2;
-    }
-  vector<uint8_t> coded;
-  for (size_t i = 0; i < n_items; i++)
-    {
-      const vector<int> bitvec = parse_payload (bits[i]);
-      if (bitvec.empty())
-        return 2;
-      const vector<uint8_t> c = gen_coded_bits (key, bitvec);
-      coded.insert (coded.end(), c.begin(), c.end());
-    }
-  awm_ctx *ctx = Engine::ctx();
-  if (!ctx || !Engine::set_embed_roles (key))
-    return 1;
-  const int limiter_block = Params::test_no_limiter ? 0 : int (sample_rate * int (Params::limiter_block_size_ms) / 1000);
-  vector<double> snr_power (2 * n_items);
-  const int rc = zero_frames
-    ? awm_embed_batch_offsets (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, zero_frames, coded.data(), Params::frames_pad_start,
-                               Params::water_delta, limiter_block, Params::limiter_ceiling, (Params::snr || stats) ? snr_power.data() : nullptr)
-    : awm_embed_batch (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), Params::frames_pad_start, Params::water_delta,
-                       limiter_block, Params::limiter_ceiling, (Params::snr || stats) ? snr_power.data() : nullptr);
-  if (rc)
-    {
-      error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
-      return 1;
-    }
-  if (stats)
-    {
-      stats->resize (n_items);
-      for (size_t i = 0; i < n_items; i++)
-        {
-          /* as add_watermark_windowed: the loop runs over the whole stream, silent prefix included */
-          const size_t n_stream = items[i].n_frames + (zero_frames ? zero_frames[i] : 0);
-          (*stats)[i] = add_stats (gen_runs (n_stream, !Params::test_no_limiter, sample_rate * int (Params::limiter_block_size_ms) / 1000),
-                                   snr_power[2 * i], snr_power[2 * i + 1]);
-        }
-    }
-  return 0;
-}
-
-int
-add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                           const vector<string>& bits, const int *sample_rates, size_t scratch_bytes, vector<AddStats> *stats,
-                           const uint64_t *zero_frames)
-{
-  char why[256];
-  if (zero_frames ? awm_batch_rates_offsets_validate (items, n_items, n_values, sample_rates, nullptr, zero_frames, Params::mark_sample_rate, why, sizeof (why))
-                  : awm_batch_rates_validate (items, n_items, n_values, sample_rates, nullptr, Params::mark_sample_rate, why, sizeof (why)))
-    {
-      error ("audiowmark: %s\n", why);
-      return 2;
-    }
-  vector<uint8_t> coded;
-  for (size_t i = 0; i < n_items; i++)
-    {
-      const vector<int> bitvec = parse_payload (bits[i]);
-      if (bitvec.empty())
-        return 2;
-      const vector<uint8_t> c = gen_coded_bits (key, bitvec);
-      coded.insert (coded.end(), c.begin(), c.end());
-    }
-  /* per item what add_watermark_buffer computes for its whole stream (silent prefix included, as add_watermark_windowed counts):
-   * frames through the mixer (other rates; counted from the item's first frame) and WatermarkGen::run calls */
-  vector<uint64_t> n_emit (n_items);
-  vector<size_t> runs (n_items);
-  for (size_t i = 0; i < n_items; i++)
-    {
-      const int rate = sample_rates[i];
-      const size_t block = size_t (rate) * size_t (Params::limiter_block_size_ms) / 1000;
-      const size_t z = zero_frames ? zero_frames[i] : 0, n_stream = z + items[i].n_frames;
-      if (rate == Params::mark_sample_rate)
-        {
-          runs[i] = gen_runs (n_stream, !Params::test_no_limiter, block);
-          continue;
-        }
-      size_t emit = 0;
-      resampled_add_plan (n_stream, rate, !Params::test_no_limiter, block, emit, runs[i]);
-      n_emit[i] = std::max<uint64_t> (emit, n_stream) - z;
-    }
-  awm_ctx *ctx = Engine::ctx();
-  if (!ctx || !Engine::set_embed_roles (key))
-    return 1;
-  vector<double> snr_power (2 * n_items);
-  const int limiter_ms = Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms);
-  double *snr = (Params::snr || stats) ? snr_power.data() : nullptr;
-  const int rc = zero_frames
-    ? awm_embed_batch_rates_offsets (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), zero_frames,
-                                     Params::mark_sample_rate, Params::frames_pad_start, Params::water_delta, limiter_ms, Params::limiter_ceiling, snr,
-                                     scratch_bytes)
-    : awm_embed_batch_rates (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), Params::mark_sample_rate,
-                             Params::frames_pad_start, Params::water_delta, limiter_ms, Params::limiter_ceiling, snr, scratch_bytes);
-  if (rc)
-    {
-      error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
-      return 1;
-    }
-  if (stats)
-    {
-      stats->resize (n_items);
-      for (size_t i = 0; i < n_items; i++)
-        (*stats)[i] = add_stats (runs[i], snr_power[2 * i], snr_power[2 * i + 1]);
-    }
-  return 0;
-}
-
-int
-add_watermark_batch_keys (const vector<Key>& keys, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                          const vector<string>& bits, const int *sample_rates, size_t scratch_bytes, vector<AddStats> *stats, const uint64_t *zero_frames)
-{
-  if (keys.size() != n_items || bits.size() != n_items)
+  const int mark = Params::mark_sample_rate;
+  if (per_item_keys && (keys.size() != n_items || bits.size() != n_items))
     {
       error ("audiowmark: %zu items but %zu keys and %zu payloads\n", n_items, keys.size(), bits.size());
       return 2;
     }
-  /* the distinct keys in order of first use; item i uses key_index[i] of them */
+  /* the distinct keys in order of first use; item i uses key_index[i] of them (0 with one key) */
   vector<uint32_t> key_index (n_items);
   vector<vector<unsigned char>> distinct;
   std::map<vector<unsigned char>, uint32_t> seen;
-  for (size_t i = 0; i < n_items; i++)
+  for (size_t i = 0; i < keys.size(); i++)
     {
       const vector<unsigned char> kb (keys[i].aes_key(), keys[i].aes_key() + Key::SIZE);
       auto it = seen.find (kb);
@@ -312,15 +191,33 @@ add_watermark_batch_keys (const vector<Key>& keys, const void *in, void *out, bo
           it = seen.emplace (kb, uint32_t (distinct.size())).first;
           distinct.push_back (kb);
         }
-      key_index[i] = it->second;
+      if (per_item_keys)
+        key_index[i] = it->second;
     }
+  /* the validator of the C call the input goes to (see awm_wm.hh), all before any GPU work */
   char why[256];
-  if (awm_batch_keys_validate (items, n_items, n_values, sample_rates, nullptr, zero_frames, key_index.data(), distinct.size(), Params::mark_sample_rate,
-                               why, sizeof (why)))
+  auto refuse = [&] { error ("audiowmark: %s\n", why); return 2; };
+  if (per_item_keys)
     {
-      error ("audiowmark: %s\n", why);
+      if (awm_batch_keys_validate (items, n_items, n_values, sample_rates, nullptr, zero_frames, key_index.data(), distinct.size(), mark, why,
+                                   sizeof (why)))
+        return refuse();
+    }
+  else if (sample_rates)
+    {
+      if (zero_frames ? awm_batch_rates_offsets_validate (items, n_items, n_values, sample_rates, nullptr, zero_frames, mark, why, sizeof (why))
+                      : awm_batch_rates_validate (items, n_items, n_values, sample_rates, nullptr, mark, why, sizeof (why)))
+        return refuse();
+    }
+  else if (zero_frames && awm_batch_offsets_validate (items, n_items, n_values, zero_frames, sample_rate, mark, why, sizeof (why)))
+    return refuse();                             // names an offset at another rate before the rate itself
+  if (!sample_rates && sample_rate != mark)
+    {
+      error ("audiowmark: batched embedding is only available at %d Hz\n", mark);
       return 2;
     }
+  if (!per_item_keys && !sample_rates && awm_batch_validate (items, n_items, n_values, why, sizeof (why)))
+    return refuse();
   /* every payload encoded with its own key's bit order, computed once per distinct key */
   const size_t n_coded = code_size (ConvBlockType::a, Params::payload_size);
   vector<vector<unsigned>> orders;
@@ -339,15 +236,16 @@ add_watermark_batch_keys (const vector<Key>& keys, const void *in, void *out, bo
       const vector<uint8_t> c = gen_coded_bits (orders[key_index[i]], bitvec);
       coded.insert (coded.end(), c.begin(), c.end());
     }
-  /* per item what the single-key call computes: frames through the mixer (other rates) and WatermarkGen::run calls */
+  /* per item what add_watermark_buffer computes for its whole stream (silent prefix included, as add_watermark_windowed counts):
+   * frames through the mixer (other rates; counted from the item's first frame) and WatermarkGen::run calls */
   vector<uint64_t> n_emit (n_items);
   vector<size_t> runs (n_items);
   for (size_t i = 0; i < n_items; i++)
     {
-      const int rate = sample_rates ? sample_rates[i] : Params::mark_sample_rate;
+      const int rate = sample_rates ? sample_rates[i] : mark;
       const size_t block = size_t (rate) * size_t (Params::limiter_block_size_ms) / 1000;
       const size_t z = zero_frames ? zero_frames[i] : 0, n_stream = z + items[i].n_frames;
-      if (rate == Params::mark_sample_rate)
+      if (rate == mark)
         {
           runs[i] = gen_runs (n_stream, !Params::test_no_limiter, block);
           continue;
@@ -359,22 +257,43 @@ add_watermark_batch_keys (const vector<Key>& keys, const void *in, void *out, bo
   awm_ctx *ctx = Engine::ctx();
   if (!ctx)
     return 1;
-  /* a call without items still needs a role set: that of the zero key, which no item reads */
-  vector<unsigned char> keys16 (std::max<size_t> (distinct.size(), 1) * Key::SIZE, 0);
-  for (size_t k = 0; k < distinct.size(); k++)
-    std::copy (distinct[k].begin(), distinct[k].end(), keys16.begin() + k * Key::SIZE);
-  const awm_role_layout layout = embed_role_layout();
-  if (awm_set_embed_roles_keys (ctx, keys16.data(), keys16.size() / Key::SIZE, &layout))
+  if (per_item_keys)
     {
-      error ("audiowmark: %s\n", awm_last_error (ctx));
-      return 1;
+      /* a call without items still needs a role set: that of the zero key, which no item reads */
+      vector<unsigned char> keys16 (std::max<size_t> (distinct.size(), 1) * Key::SIZE, 0);
+      for (size_t k = 0; k < distinct.size(); k++)
+        std::copy (distinct[k].begin(), distinct[k].end(), keys16.begin() + k * Key::SIZE);
+      const awm_role_layout layout = embed_role_layout();
+      if (awm_set_embed_roles_keys (ctx, keys16.data(), keys16.size() / Key::SIZE, &layout))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return 1;
+        }
     }
+  else if (!Engine::set_embed_roles (keys[0]))
+    return 1;
   vector<double> snr_power (2 * n_items);
-  const int limiter_ms = Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms);
   double *snr = (Params::snr || stats) ? snr_power.data() : nullptr;
-  if (awm_embed_batch_keys (ctx, in, out, s16 ? 1 : 0, n_values, items, n_items, coded.data(), sample_rates, sample_rates ? n_emit.data() : nullptr,
-                            zero_frames, key_index.data(), Params::mark_sample_rate, Params::frames_pad_start, Params::water_delta, limiter_ms,
-                            Params::limiter_ceiling, snr, scratch_bytes))
+  const int limiter_ms = Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms);
+  const int limiter_block = limiter_ms * mark / 1000;
+  const int is_s16 = s16 ? 1 : 0, pad = Params::frames_pad_start;
+  const double wd = Params::water_delta;
+  const float ceiling = Params::limiter_ceiling;
+  int rc;
+  if (per_item_keys)
+    rc = awm_embed_batch_keys (ctx, in, out, is_s16, n_values, items, n_items, coded.data(), sample_rates, sample_rates ? n_emit.data() : nullptr,
+                               zero_frames, key_index.data(), mark, pad, wd, limiter_ms, ceiling, snr, scratch_bytes);
+  else if (sample_rates && zero_frames)
+    rc = awm_embed_batch_rates_offsets (ctx, in, out, is_s16, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), zero_frames, mark,
+                                        pad, wd, limiter_ms, ceiling, snr, scratch_bytes);
+  else if (sample_rates)
+    rc = awm_embed_batch_rates (ctx, in, out, is_s16, n_values, items, n_items, coded.data(), sample_rates, n_emit.data(), mark, pad, wd, limiter_ms,
+                                ceiling, snr, scratch_bytes);
+  else if (zero_frames)
+    rc = awm_embed_batch_offsets (ctx, in, out, is_s16, n_values, items, n_items, zero_frames, coded.data(), pad, wd, limiter_block, ceiling, snr);
+  else
+    rc = awm_embed_batch (ctx, in, out, is_s16, n_values, items, n_items, coded.data(), pad, wd, limiter_block, ceiling, snr);
+  if (rc)
     {
       error ("audiowmark: batched embedding failed: %s\n", awm_last_error (ctx));
       return 1;

@@ -260,135 +260,27 @@ awmh_add (const unsigned char *key16, const float *in, float *out, size_t n_fram
   return rc;
 }
 
-/* add_watermark_batch on a packed buffer (float or 16 bit PCM, host or device): payload_hex[i] goes into items[i];
- * data_blocks / snr_db (optional): [n_items].  Returns 2 for a malformed item list (checked before any GPU work). */
-static int
-add_batch_any (const unsigned char *key16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-               const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db, const uint64_t *zero_frames = nullptr)
-{
-  std::vector<std::string> bits (n_items);
-  for (size_t i = 0; i < n_items; i++)
-    bits[i] = payload_hex[i] ? payload_hex[i] : "";
-  std::vector<AddStats> stats;
-  const int rc = add_watermark_batch (make_key (key16, ""), in, out, s16, n_values, items, n_items, bits, sample_rate,
-                                      (data_blocks || snr_db) ? &stats : nullptr, zero_frames);
-  for (size_t i = 0; i < stats.size(); i++)
-    {
-      if (data_blocks)
-        data_blocks[i] = stats[i].data_blocks;
-      if (snr_db)
-        snr_db[i] = stats[i].snr_db;
-    }
-  return rc;
-}
-
+/* add_watermark_batch on a packed buffer (is_s16: 16 bit PCM, else float; host or device): payload_hex[i] goes into items[i].
+ * keys16: one 16-byte key, or with per_item_keys [n_items][16] with item i's key.  sample_rates (NULL: every item is at sample_rate)
+ * and zero_frames (NULL: every item starts its stream): [n_items].  data_blocks / snr_db (optional): [n_items].  Returns 2 for
+ * malformed input (checked before any GPU work), 1 for other errors. */
 int
-awmh_add_batch (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
+awmh_add_batch (const unsigned char *keys16, int per_item_keys, const void *in, void *out, int is_s16, size_t n_values, const awm_batch_item *items,
+                size_t n_items, const char *const *payload_hex, int sample_rate, const int *sample_rates, const uint64_t *zero_frames,
+                size_t scratch_bytes, int *data_blocks, double *snr_db)
 {
-  return add_batch_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db);
-}
-
-int
-awmh_add_batch_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                    const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
-{
-  return add_batch_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db);
-}
-
-/* add_watermark_batch with stream offsets: items[i] continues a stream that began zero_frames[i] frames earlier with silence (an HLS
- * segment; zero_frames NULL: all zero); otherwise as awmh_add_batch.  Returns 2 for a malformed offset list too
- * (awm_batch_offsets_validate). */
-int
-awmh_add_batch_offsets (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                        const uint64_t *zero_frames, const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
-{
-  return add_batch_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db, zero_frames);
-}
-
-int
-awmh_add_batch_offsets_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                            const uint64_t *zero_frames, const char *const *payload_hex, int sample_rate, int *data_blocks, double *snr_db)
-{
-  return add_batch_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rate, data_blocks, snr_db, zero_frames);
-}
-
-/* add_watermark_batch_rates on a packed buffer: items[i] is at sample_rates[i]; otherwise as awmh_add_batch */
-static int
-add_batch_rates_any (const unsigned char *key16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                     const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db,
-                     const uint64_t *zero_frames = nullptr)
-{
-  std::vector<std::string> bits (n_items);
-  for (size_t i = 0; i < n_items; i++)
-    bits[i] = payload_hex[i] ? payload_hex[i] : "";
-  std::vector<AddStats> stats;
-  const int rc = add_watermark_batch_rates (make_key (key16, ""), in, out, s16, n_values, items, n_items, bits, sample_rates, scratch_bytes,
-                                            (data_blocks || snr_db) ? &stats : nullptr, zero_frames);
-  for (size_t i = 0; i < stats.size(); i++)
-    {
-      if (data_blocks)
-        data_blocks[i] = stats[i].data_blocks;
-      if (snr_db)
-        snr_db[i] = stats[i].snr_db;
-    }
-  return rc;
-}
-
-int
-awmh_add_batch_rates (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                      const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db)
-{
-  return add_batch_rates_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
-}
-
-int
-awmh_add_batch_rates_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                          const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks, double *snr_db)
-{
-  return add_batch_rates_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
-}
-
-/* add_watermark_batch_rates with stream offsets: items[i] continues a stream at sample_rates[i] that began zero_frames[i] frames (at
- * that rate) earlier with silence (an HLS segment of a 48 kHz master); otherwise as awmh_add_batch_rates.  Returns 2 for a malformed
- * offset list too (awm_batch_rates_offsets_validate). */
-int
-awmh_add_batch_rates_offsets (const unsigned char *key16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                              const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes,
-                              int *data_blocks, double *snr_db)
-{
-  return add_batch_rates_any (key16, in, out, false, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db,
-                              zero_frames);
-}
-
-int
-awmh_add_batch_rates_offsets_s16 (const unsigned char *key16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items,
-                                  size_t n_items, const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates,
-                                  size_t scratch_bytes, int *data_blocks, double *snr_db)
-{
-  return add_batch_rates_any (key16, in, out, true, n_values, items, n_items, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db,
-                              zero_frames);
-}
-
-/* add_watermark_batch_keys on a packed buffer: keys16 [n_items][16] holds item i's key; zero_frames and sample_rates may be NULL
- * (every item starts its stream / is at 44.1 kHz); otherwise as awmh_add_batch_rates_offsets.  Returns 2 on malformed input. */
-static int
-add_batch_keys_any (const unsigned char *keys16, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                    const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks,
-                    double *snr_db)
-{
-  if (n_items && (!keys16 || !payload_hex))
+  const size_t n_keys = per_item_keys ? n_items : 1;
+  if ((n_keys && !keys16) || (n_items && !payload_hex))
     return 2;
-  std::vector<Key> keys (n_items);
+  std::vector<Key> keys (n_keys);
+  for (size_t i = 0; i < n_keys; i++)
+    keys[i] = make_key (keys16 + i * Key::SIZE, "");
   std::vector<std::string> bits (n_items);
   for (size_t i = 0; i < n_items; i++)
-    {
-      keys[i] = make_key (keys16 + i * Key::SIZE, "");
-      bits[i] = payload_hex[i] ? payload_hex[i] : "";
-    }
+    bits[i] = payload_hex[i] ? payload_hex[i] : "";
   std::vector<AddStats> stats;
-  const int rc = add_watermark_batch_keys (keys, in, out, s16, n_values, items, n_items, bits, sample_rates, scratch_bytes,
-                                           (data_blocks || snr_db) ? &stats : nullptr, zero_frames);
+  const int rc = add_watermark_batch (keys, per_item_keys != 0, in, out, is_s16 != 0, n_values, items, n_items, bits, sample_rate, sample_rates,
+                                      zero_frames, scratch_bytes, (data_blocks || snr_db) ? &stats : nullptr);
   for (size_t i = 0; i < stats.size(); i++)
     {
       if (data_blocks)
@@ -397,22 +289,6 @@ add_batch_keys_any (const unsigned char *keys16, const void *in, void *out, bool
         snr_db[i] = stats[i].snr_db;
     }
   return rc;
-}
-
-int
-awmh_add_batch_keys (const unsigned char *keys16, const float *in, float *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                     const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks,
-                     double *snr_db)
-{
-  return add_batch_keys_any (keys16, in, out, false, n_values, items, n_items, zero_frames, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
-}
-
-int
-awmh_add_batch_keys_s16 (const unsigned char *keys16, const int16_t *in, int16_t *out, size_t n_values, const awm_batch_item *items, size_t n_items,
-                         const uint64_t *zero_frames, const char *const *payload_hex, const int *sample_rates, size_t scratch_bytes, int *data_blocks,
-                         double *snr_db)
-{
-  return add_batch_keys_any (keys16, in, out, true, n_values, items, n_items, zero_frames, payload_hex, sample_rates, scratch_bytes, data_blocks, snr_db);
 }
 
 /* the role layout of the current Params (what awm_set_embed_roles_keys takes) as 6 ints in awm_role_layout's field order */

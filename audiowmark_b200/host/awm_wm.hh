@@ -20,31 +20,21 @@ int add_watermark_buffer (const Key& key, const float *in, float *out, size_t n_
                           const std::string& bits, AddStats *stats, uint64_t first_frame_number = 0);
 
 /* add_watermark_buffer for many items of one packed buffer (float or 16 bit PCM, host or device), one payload per item, in one pass
- * over the GPU; item i comes out bit identical to add_watermark_buffer[_s16] on it alone.  44.1 kHz only.  stats (optional) gets
- * one entry per item.  zero_frames (optional, [n_items]): item i continues a stream that began zero_frames[i] frames earlier with
- * silence (HLS segments): it comes out as add_watermark_windowed with that zero_frames, its stats as that call reports them.
- * Returns 2 for a malformed item list, offset list or payload, 1 for other errors. */
-int add_watermark_batch (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                         const std::vector<std::string>& bits, int sample_rate, std::vector<AddStats> *stats, const uint64_t *zero_frames = nullptr);
-
-/* add_watermark_batch for items that each have their own sample rate (sample_rates[i]): item i comes out bit identical to
- * add_watermark_buffer on it alone at that rate (16 bit items: converted to float and back around it, as `audiowmark add` does for a
- * 16 bit file).  scratch_bytes: awm_embed_batch_rates's wave size, 0 = its default.  zero_frames (optional, [n_items], frames at the
- * item's own rate): item i continues a stream that began zero_frames[i] frames earlier with silence: it comes out as
- * add_watermark_buffer of zeros (z) ++ item with the first z frames dropped, Data Blocks counted over that stream, --snr over the
- * item's own positions.  Returns 2 for a malformed item list, rate, offset list or payload, 1 for other errors. */
-int add_watermark_batch_rates (const Key& key, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items, size_t n_items,
-                               const std::vector<std::string>& bits, const int *sample_rates, size_t scratch_bytes, std::vector<AddStats> *stats,
-                               const uint64_t *zero_frames = nullptr);
-
-/* add_watermark_batch_rates with a key per item (keys[i] for item i, keys.size() == n_items): item i comes out bit identical to the
- * single-key batch call with keys[i], its stats as that call reports them.  sample_rates NULL: every item is at 44.1 kHz;
- * zero_frames (optional) as in add_watermark_batch_rates.  The role tables of the distinct keys are built on the device once per call
- * (awm_set_embed_roles_keys), each payload is encoded with its own key's bit order.  Returns 2 for a malformed item list, key list,
- * rate, offset list or payload, 1 for other errors. */
-int add_watermark_batch_keys (const std::vector<Key>& keys, const void *in, void *out, bool s16, size_t n_values, const awm_batch_item *items,
-                              size_t n_items, const std::vector<std::string>& bits, const int *sample_rates, size_t scratch_bytes,
-                              std::vector<AddStats> *stats, const uint64_t *zero_frames = nullptr);
+ * over the GPU; item i comes out bit identical to add_watermark_buffer[_s16] on it alone, stats (optional) gets one entry per item.
+ *   keys: one key for every item, or with per_item_keys keys[i] for item i (keys.size() == n_items; the role tables of the distinct
+ *     keys are built on the device once per call, each payload is encoded with its own key's bit order).
+ *   sample_rates (optional, [n_items]): item i is at sample_rates[i] (16 bit items: converted to float and back around the add, as
+ *     `audiowmark add` does for a 16 bit file).  Without it every item is at sample_rate, which must be 44.1 kHz.
+ *   zero_frames (optional, [n_items], frames at the item's own rate): item i continues a stream that began zero_frames[i] frames
+ *     earlier with silence (HLS segments): it comes out as add_watermark_buffer of zeros (z) ++ item with the first z frames dropped,
+ *     Data Blocks counted over that stream, --snr over the item's own positions.
+ *   scratch_bytes: the wave size of the calls with a rate list, 0 = their default.
+ * The input picks the C call, and each call runs its own k_embed_batch instance:
+ *   per-item keys: awm_embed_batch_keys;  one key: awm_embed_batch, _offsets, _rates or _rates_offsets by which lists are given.
+ * Returns 2 for a malformed item list, key list, rate, offset list or payload (before any GPU work), 1 for other errors. */
+int add_watermark_batch (const std::vector<Key>& keys, bool per_item_keys, const void *in, void *out, bool s16, size_t n_values,
+                         const awm_batch_item *items, size_t n_items, const std::vector<std::string>& bits, int sample_rate, const int *sample_rates,
+                         const uint64_t *zero_frames, size_t scratch_bytes, std::vector<AddStats> *stats);
 
 /* add_stream_watermark's loop with bounded memory (window by window; see awm_add.cc); callbacks read / write interleaved frames */
 int add_watermark_windowed (const Key& key, const std::function<Error (std::vector<float>&, size_t)>& read,

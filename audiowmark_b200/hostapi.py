@@ -17,9 +17,7 @@ CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
            "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_bg_input_range", "awmh_add_windowed",
-           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_add_batch_s16", "awmh_add_batch_rates", "awmh_add_batch_rates_s16",
-           "awmh_add_batch_offsets", "awmh_add_batch_offsets_s16", "awmh_add_batch_rates_offsets", "awmh_add_batch_rates_offsets_s16",
-           "awmh_add_batch_keys", "awmh_add_batch_keys_s16", "awmh_role_layout", "awmh_embed_roles_device"]
+           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_role_layout", "awmh_embed_roles_device"]
 
 _lib = None
 
@@ -164,17 +162,6 @@ def _keys(keys, name, n=None) -> bytes:
     return b"".join(kb)
 
 
-def _add_batch_keys(name, keys, key, s16, it, n_values, p_in, p_out, z, payloads, rates, scratch_bytes, stats):
-    """awmh_add_batch_keys[_s16] for add_batch / add_batch_rates with keys=; rates None: every item at 44.1 kHz"""
-    if key is not None:
-        raise ValueError("%s: pass either key= or keys=, not both" % name)
-    kb = _keys(keys, name, len(it))
-    pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
-    fn = load().awmh_add_batch_keys_s16 if s16 else load().awmh_add_batch_keys
-    return fn(kb if kb else None, p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), _ptr(z), pay, _ptr(rates),
-              ctypes.c_size_t(scratch_bytes), *stats)
-
-
 def coded_bits(key, payload_hex: str) -> np.ndarray:
     """one payload's coded data bits uint8 [2 (A, B), n_coded]: randomize_bit_order (code_encode (A | B, payload))"""
     out = np.zeros((2, n_coded_bits()), np.uint8)
@@ -273,6 +260,41 @@ def _zero_frames(name, zero_frames, n_items):
     return np.array([int(v) for v in z], np.uint64)
 
 
+def _add_batch(name, pcms, payloads, key, keys, items, out, want_stats, zero_frames, sample_rate=44100, sample_rates=None, scratch_bytes=0):
+    """add_batch, or add_batch_rates when sample_rates is given, through awmh_add_batch"""
+    payloads = list(payloads)
+    rates = None if sample_rates is None else np.array([int(r) for r in sample_rates], np.int64)
+    s16, it, n_values, p_in, p_out, split, _keep = _pack_batch(name, pcms, payloads, items, out)
+    if rates is not None:
+        if len(rates) != len(it):
+            raise ValueError("%s: %d items but %d sample rates" % (name, len(it), len(rates)))
+        if np.any(rates <= 0) or np.any(rates > np.iinfo(np.int32).max):
+            raise ValueError("%s: sample rates must be positive 32 bit integers" % name)
+        rates = np.ascontiguousarray(rates, np.int32)
+    z = None if zero_frames is None else _zero_frames(name, zero_frames, len(it))
+    if keys is None:
+        kb = _key(key)
+    else:
+        if rates is None and sample_rate != 44100:
+            raise ValueError("%s: only 44.1 kHz input is accepted (use add_batch_rates)" % name)
+        if key is not None:
+            raise ValueError("%s: pass either key= or keys=, not both" % name)
+        kb = _keys(keys, name, len(it))
+    pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
+    blocks = np.zeros(max(len(it), 1), np.int32)
+    snr = np.zeros(max(len(it), 1), np.float64)
+    rc = load().awmh_add_batch(kb or None, ctypes.c_int(keys is not None), p_in, p_out, ctypes.c_int(s16), ctypes.c_size_t(n_values), _ptr(it),
+                               ctypes.c_size_t(len(it)), pay, ctypes.c_int(sample_rate), _ptr(rates), _ptr(z), ctypes.c_size_t(scratch_bytes),
+                               _ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
+    if rc == 2:
+        raise ValueError("%s: malformed item list, %soffset list or payload; see stderr" % (name, "" if rates is None else "sample rate, "))
+    if rc:
+        raise RuntimeError("awmh_add_batch failed (rc=%d); see stderr" % rc)
+    synchronize()
+    outs = [split(int(t["value_offset"]), int(t["n_frames"]), int(t["channels"])) for t in it]
+    return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs
+
+
 def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None, want_stats=False, zero_frames=None, keys=None):
     """`add` for many items with one key and one payload each, in one pass over the GPU; item i comes out bit identical to
     add / add_s16 of that item alone with payloads[i].
@@ -287,31 +309,7 @@ def add_batch(pcms, payloads, key=None, sample_rate=44100, items=None, out=None,
             role tables of the distinct keys are built on the device in one launch.
     Returns the list of outputs (numpy arrays, or views of the output tensor), with want_stats also the lists of data blocks
     and SNR dB per item.  Only 44.1 kHz input is accepted.  Raises ValueError for a malformed item list, offset list or payload."""
-    payloads = list(payloads)
-    s16, it, n_values, p_in, p_out, split, _keep = _pack_batch("add_batch", pcms, payloads, items, out)
-    z = None if zero_frames is None else _zero_frames("add_batch", zero_frames, len(it))
-    pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
-    blocks = np.zeros(max(len(it), 1), np.int32)
-    snr = np.zeros(max(len(it), 1), np.float64)
-    stats = (_ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
-    if keys is not None:
-        if sample_rate != 44100:
-            raise ValueError("add_batch: only 44.1 kHz input is accepted (use add_batch_rates)")
-        rc = _add_batch_keys("add_batch", keys, key, s16, it, n_values, p_in, p_out, z, payloads, None, 0, stats)
-    elif z is None:
-        fn = load().awmh_add_batch_s16 if s16 else load().awmh_add_batch
-        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, ctypes.c_int(sample_rate), *stats)
-    else:
-        fn = load().awmh_add_batch_offsets_s16 if s16 else load().awmh_add_batch_offsets
-        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), _ptr(z), pay, ctypes.c_int(sample_rate),
-                *stats)
-    if rc == 2:
-        raise ValueError("add_batch: malformed item list, offset list or payload; see stderr")
-    if rc:
-        raise RuntimeError("awmh_add_batch failed (rc=%d); see stderr" % rc)
-    synchronize()
-    outs = [split(int(t["value_offset"]), int(t["n_frames"]), int(t["channels"])) for t in it]
-    return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs
+    return _add_batch("add_batch", pcms, payloads, key, keys, items, out, want_stats, zero_frames, sample_rate=sample_rate)
 
 
 def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None, want_stats=False, scratch_bytes=0, zero_frames=None, keys=None):
@@ -325,36 +323,8 @@ def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None
     the silent prefix is never allocated.  zero_frames + n_frames is limited to 2^48 per item, at the item's rate and at 44.1 kHz.
     keys: None, or one 16-byte key per item (instead of key=), as in add_batch.
     Raises ValueError for a malformed item list, rate list, offset list or payload."""
-    payloads = list(payloads)
-    rates = np.array([int(r) for r in sample_rates], np.int64)
-    s16, it, n_values, p_in, p_out, split, _keep = _pack_batch("add_batch_rates", pcms, payloads, items, out)
-    if len(rates) != len(it):
-        raise ValueError("add_batch_rates: %d items but %d sample rates" % (len(it), len(rates)))
-    if np.any(rates <= 0) or np.any(rates > np.iinfo(np.int32).max):
-        raise ValueError("add_batch_rates: sample rates must be positive 32 bit integers")
-    rates = np.ascontiguousarray(rates, np.int32)
-    z = None if zero_frames is None else _zero_frames("add_batch_rates", zero_frames, len(it))
-    pay = (ctypes.c_char_p * max(len(payloads), 1))(*[p.encode() for p in payloads])
-    blocks = np.zeros(max(len(it), 1), np.int32)
-    snr = np.zeros(max(len(it), 1), np.float64)
-    stats = (_ptr(blocks) if want_stats else None, _ptr(snr) if want_stats else None)
-    if keys is not None:
-        rc = _add_batch_keys("add_batch_rates", keys, key, s16, it, n_values, p_in, p_out, z, payloads, rates, scratch_bytes, stats)
-    elif z is None:
-        fn = load().awmh_add_batch_rates_s16 if s16 else load().awmh_add_batch_rates
-        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), pay, _ptr(rates),
-                ctypes.c_size_t(scratch_bytes), *stats)
-    else:
-        fn = load().awmh_add_batch_rates_offsets_s16 if s16 else load().awmh_add_batch_rates_offsets
-        rc = fn(_key(key), p_in, p_out, ctypes.c_size_t(n_values), _ptr(it), ctypes.c_size_t(len(it)), _ptr(z), pay, _ptr(rates),
-                ctypes.c_size_t(scratch_bytes), *stats)
-    if rc == 2:
-        raise ValueError("add_batch_rates: malformed item list, sample rate, offset list or payload; see stderr")
-    if rc:
-        raise RuntimeError("awmh_add_batch_rates failed (rc=%d); see stderr" % rc)
-    synchronize()
-    outs = [split(int(t["value_offset"]), int(t["n_frames"]), int(t["channels"])) for t in it]
-    return (outs, blocks[:len(it)].tolist(), snr[:len(it)].tolist()) if want_stats else outs
+    return _add_batch("add_batch_rates", pcms, payloads, key, keys, items, out, want_stats, zero_frames, sample_rates=sample_rates,
+                      scratch_bytes=scratch_bytes)
 
 
 def add_windowed(pcm_in: np.ndarray, payload_hex: str, key=None, zero_frames=0, window_frames=0, sample_rate=44100):

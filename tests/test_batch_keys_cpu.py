@@ -1,6 +1,6 @@
-"""CPU: the batched embed with a key per item (hostapi.add_batch / add_batch_rates with keys= -> awmh_add_batch_keys ->
-awm_batch_keys_validate).  The validator accepts what the matching single-key validator accepts and, in addition, needs a key index
-below the role set's key count for every item; malformed calls are rejected with ValueError before any GPU work."""
+"""CPU: the batched embed with a key per item (hostapi.add_batch / add_batch_rates with keys= -> awmh_add_batch with per-item
+keys -> awm_batch_keys_validate).  The validator accepts what the matching single-key validator accepts and, in addition, needs a
+key index below the role set's key count for every item; malformed calls are rejected with ValueError before any GPU work."""
 import ctypes
 
 import numpy as np

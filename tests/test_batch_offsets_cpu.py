@@ -1,6 +1,6 @@
-"""CPU: input checks of the batched embed at stream offsets (hostapi.add_batch(zero_frames=...) -> awmh_add_batch_offsets ->
-awm_batch_offsets_validate).  Every malformed offset list is rejected with ValueError (rc 2 from the host exports) before any GPU
-work; well-formed input gets as far as the device and fails there with RuntimeError when there is none."""
+"""CPU: input checks of the batched embed at stream offsets (hostapi.add_batch(zero_frames=...) -> awmh_add_batch with an offset
+list -> awm_batch_offsets_validate).  Every malformed offset list is rejected with ValueError (rc 2 from the host export) before
+any GPU work; well-formed input gets as far as the device and fails there with RuntimeError when there is none."""
 import os
 
 import numpy as np
@@ -53,7 +53,7 @@ def test_add_batch_rejects_bad_offsets_before_gpu_work():
         H.add_batch(x16, [T.PAYLOAD, T.PAYLOAD], zero_frames=[0, LIMIT])             # the 16 bit entry point checks the same way
 
 
-def test_host_exports_return_2_for_malformed_offsets():
+def test_host_export_returns_2_for_malformed_offsets():
     lib = H.load()
     buf = np.zeros(100, np.float32)
     out = np.zeros_like(buf)
@@ -61,12 +61,12 @@ def test_host_exports_return_2_for_malformed_offsets():
     it = np.array([(0, 10, 2)], capi.BATCH_ITEM)
     for z, rate in (([LIMIT], 44100), ([2 ** 64 - 1], 44100), ([1], 32000)):
         zf = np.array(z, np.uint64)
-        rc = lib.awmh_add_batch_offsets(H._key(None), H._ptr(buf), H._ptr(out), H.ctypes.c_size_t(buf.size), H._ptr(it), H.ctypes.c_size_t(1),
-                                        H._ptr(zf), pay, H.ctypes.c_int(rate), None, None)
+        rc = lib.awmh_add_batch(H._key(None), 0, H._ptr(buf), H._ptr(out), 0, H.ctypes.c_size_t(buf.size), H._ptr(it), H.ctypes.c_size_t(1),
+                                pay, H.ctypes.c_int(rate), None, H._ptr(zf), H.ctypes.c_size_t(0), None, None)
         assert rc == 2, (z, rate)
         b16 = np.zeros(100, np.int16)
-        rc = lib.awmh_add_batch_offsets_s16(H._key(None), H._ptr(b16), H._ptr(np.zeros_like(b16)), H.ctypes.c_size_t(b16.size), H._ptr(it),
-                                            H.ctypes.c_size_t(1), H._ptr(zf), pay, H.ctypes.c_int(rate), None, None)
+        rc = lib.awmh_add_batch(H._key(None), 0, H._ptr(b16), H._ptr(np.zeros_like(b16)), 1, H.ctypes.c_size_t(b16.size), H._ptr(it),
+                                H.ctypes.c_size_t(1), pay, H.ctypes.c_int(rate), None, H._ptr(zf), H.ctypes.c_size_t(0), None, None)
         assert rc == 2, (z, rate)
 
 

@@ -1,4 +1,4 @@
-"""CPU: input checks of the batched embed at any sample rate (hostapi.add_batch_rates -> awmh_add_batch_rates ->
+"""CPU: input checks of the batched embed at any sample rate (hostapi.add_batch_rates -> awmh_add_batch with a rate list ->
 awm_batch_rates_validate).  Every malformed call is rejected with ValueError before any GPU work; well-formed input gets as far as
 the device and fails there with RuntimeError when there is none."""
 import os
@@ -53,7 +53,7 @@ def test_add_batch_rates_rejects_bad_input_before_gpu_work():
         H.add_batch_rates(x16, [T.PAYLOAD, T.PAYLOAD], [48000, 5])           # the 16 bit entry point checks the same way
 
 
-def test_add_batch_rates_rejects_malformed_item_list():
+def test_host_export_returns_2_for_malformed_rate_items():
     lib = H.load()
     buf = np.zeros(100, np.float32)
     out = np.zeros_like(buf)
@@ -61,8 +61,8 @@ def test_add_batch_rates_rejects_malformed_item_list():
     rates = np.array([48000], np.int32)
     for items in ([(0, 10, 0)], [(0, 60, 2)], [(101, 0, 1)]):
         it = np.array(items, capi.BATCH_ITEM)
-        rc = lib.awmh_add_batch_rates(H._key(None), H._ptr(buf), H._ptr(out), H.ctypes.c_size_t(buf.size), H._ptr(it), H.ctypes.c_size_t(1),
-                                      pay, H._ptr(rates), H.ctypes.c_size_t(0), None, None)
+        rc = lib.awmh_add_batch(H._key(None), 0, H._ptr(buf), H._ptr(out), 0, H.ctypes.c_size_t(buf.size), H._ptr(it), H.ctypes.c_size_t(1),
+                                pay, 44100, H._ptr(rates), None, H.ctypes.c_size_t(0), None, None)
         assert rc == 2, items
 
 

@@ -1,7 +1,7 @@
-"""CPU: the batched embed at stream positions at any sample rate (hostapi.add_batch_rates(zero_frames=...) ->
-awmh_add_batch_rates_offsets -> awm_batch_rates_offsets_validate), and the add loop's frame counts (resampled_add_plan) that every
-item's stream needs.  Malformed offset lists are rejected with ValueError (rc 2 from the host exports) before any GPU work; the
-plan is the old per-1024-frame loop's result, in time that does not grow with the stream."""
+"""CPU: the batched embed at stream positions at any sample rate (hostapi.add_batch_rates(zero_frames=...) -> awmh_add_batch with
+rate and offset lists -> awm_batch_rates_offsets_validate), and the add loop's frame counts (resampled_add_plan) that every item's
+stream needs.  Malformed offset lists are rejected with ValueError (rc 2 from the host export) before any GPU work; the plan is
+the old per-1024-frame loop's result, in time that does not grow with the stream."""
 import os
 import time
 
@@ -79,7 +79,7 @@ def test_add_batch_rates_rejects_bad_offsets_before_gpu_work():
         H.add_batch_rates(x16, [T.PAYLOAD, T.PAYLOAD], [48000, 32000], zero_frames=[0, LIMIT])
 
 
-def test_host_exports_return_2_for_malformed_offsets():
+def test_host_export_returns_2_for_malformed_rate_offsets():
     lib = H.load()
     buf = np.zeros(100, np.float32)
     pay = (H.ctypes.c_char_p * 1)(T.PAYLOAD.encode())
@@ -87,12 +87,12 @@ def test_host_exports_return_2_for_malformed_offsets():
     for z, rate in (([LIMIT], 48000), ([2 ** 64 - 1], 44100), ([LIMIT // 5], 8000)):
         zf = np.array(z, np.uint64)
         rates = np.array([rate], np.int32)
-        rc = lib.awmh_add_batch_rates_offsets(H._key(None), H._ptr(buf), H._ptr(np.zeros_like(buf)), H.ctypes.c_size_t(buf.size), H._ptr(it),
-                                              H.ctypes.c_size_t(1), H._ptr(zf), pay, H._ptr(rates), H.ctypes.c_size_t(0), None, None)
+        rc = lib.awmh_add_batch(H._key(None), 0, H._ptr(buf), H._ptr(np.zeros_like(buf)), 0, H.ctypes.c_size_t(buf.size), H._ptr(it),
+                                H.ctypes.c_size_t(1), pay, 44100, H._ptr(rates), H._ptr(zf), H.ctypes.c_size_t(0), None, None)
         assert rc == 2, (z, rate)
         b16 = np.zeros(100, np.int16)
-        rc = lib.awmh_add_batch_rates_offsets_s16(H._key(None), H._ptr(b16), H._ptr(np.zeros_like(b16)), H.ctypes.c_size_t(b16.size), H._ptr(it),
-                                                  H.ctypes.c_size_t(1), H._ptr(zf), pay, H._ptr(rates), H.ctypes.c_size_t(0), None, None)
+        rc = lib.awmh_add_batch(H._key(None), 0, H._ptr(b16), H._ptr(np.zeros_like(b16)), 1, H.ctypes.c_size_t(b16.size), H._ptr(it),
+                                H.ctypes.c_size_t(1), pay, 44100, H._ptr(rates), H._ptr(zf), H.ctypes.c_size_t(0), None, None)
         assert rc == 2, (z, rate)
 
 
