@@ -36,7 +36,7 @@ EXPORTS = [
     "awm_set_embed_roles_keys", "awm_get_embed_roles_keys", "awm_batch_keys_validate", "awm_embed_batch_keys",
     "awm_speed_mags", "awm_resampler_cache",
     "awm_resample_stream_available", "awm_resample_stream_frames", "awm_resample_taps", "awm_resample_range_validate", "awm_resample_range",
-    "awm_device_alloc", "awm_device_free",
+    "awm_device_alloc", "awm_device_free", "awm_embed_window_rates", "awm_window_range_rates",
 ]
 
 _lib = None
@@ -146,6 +146,18 @@ def resample_taps(n_in_total: int, ratio: float, out_first: int, out_frames: int
     first, end = ctypes.c_uint64(), ctypes.c_uint64()
     load().awm_resample_taps(ctypes.c_uint64(n_in_total), ctypes.c_double(ratio), ctypes.c_int(hlen), ctypes.c_uint64(out_first),
                              ctypes.c_uint64(out_frames), ctypes.byref(first), ctypes.byref(end))
+    return first.value, end.value
+
+
+def window_range_rates(own_first: int, own_end: int, n_total: int, sample_rate: int, mark_sample_rate: int = 44100, limiter_ms: int = 1000,
+                       hlen: int = 16) -> tuple[int, int]:
+    """awm_window_range_rates: input frames [ext_first, ext_end) that make awm_embed_window_rates's outputs [own_first, own_end) exact
+    (n_total = 2^64-1: the end is not known yet); ValueError for a range or rate the planner refuses"""
+    first, end = ctypes.c_uint64(), ctypes.c_uint64()
+    rc = load().awm_window_range_rates(ctypes.c_uint64(own_first), ctypes.c_uint64(own_end), ctypes.c_uint64(n_total), ctypes.c_int(sample_rate),
+                                       ctypes.c_int(mark_sample_rate), ctypes.c_int(limiter_ms), ctypes.c_int(hlen), ctypes.byref(first), ctypes.byref(end))
+    if rc:
+        raise ValueError("awm_window_range_rates refuses own [%d, %d) of %d frames at %d Hz" % (own_first, own_end, n_total, sample_rate))
     return first.value, end.value
 
 

@@ -41,6 +41,7 @@ struct RateItem
   long long w0;                // stream position (watermark rate) of the scratch's first frame, a multiple of 1024
   long long i0;                // first stream position (input rate) whose watermark can be non-zero, <= z
   long long blk0;              // i0 / limiter_block: the limiter block of peaks[peak0]
+  long long snr0, snr1;        // stream positions [snr0, snr1) the --snr sums count (OFFSETS only): [z, z + n_emit) unless a window narrows them
 };
 
 constexpr int kRateCta = 256;  // threads (= output frames) per resampling CTA
@@ -108,7 +109,7 @@ k_resample_batch (const RateItem *__restrict__ items, int n_items)
 // frame i < n_emit of an item: y = wm + orig (orig is zero beyond n_frames), stored for i < n_frames; peak of |y| per limiter block
 // of the item (only peaks above the ceiling matter, Limiter::block_max starts at the ceiling); --snr sums of wm and orig.  The
 // watermark is resampled by the operations of k_resample and stays in registers.  OFFSETS: stream position i = i0 + thread's frame
-// is the item's frame i - z; positions before z are neither stored nor summed for --snr.
+// is the item's frame i - z; positions before z are not stored, and only positions in [snr0, snr1) are summed for --snr.
 template<bool OFFSETS> __global__ void __launch_bounds__ (kRateCta)
 k_resample_mix_batch (const RateItem *__restrict__ items, int n_items, float ceiling, unsigned *__restrict__ peaks, double *__restrict__ snr)
 {
@@ -127,7 +128,7 @@ k_resample_mix_batch (const RateItem *__restrict__ items, int n_items, float cei
   const long long q = OFFSETS ? i - it.z : i;               // frame of the item
   const int C = it.C;
   const bool own = OFFSETS ? q >= 0 && q < it.n_frames : i < it.n_frames;
-  const bool counts = !OFFSETS || q >= 0;                   // --snr: the item's own positions
+  const bool counts = !OFFSETS || (i >= it.snr0 && i < it.snr1);   // --snr: the item's own positions, or a window's owned part
   double sd = 0, ss = 0;
   if (k < J.n_out)
     {

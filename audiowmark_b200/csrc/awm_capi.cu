@@ -2974,12 +2974,14 @@ namespace {
  * own argument checks (name: the error prefix).  sample_rates NULL: every item is at mark_sample_rate; zero_frames NULL: every item
  * starts a stream; key_index NULL: every item uses the role table of awm_set_embed_roles, else item i that of key key_index[i] of
  * the role set of awm_set_embed_roles_keys.  Items at mark_sample_rate use limiter_block44, the others rate * limiter_ms / 1000;
- * n_emit[i] counts from the item's first frame. */
+ * n_emit[i] counts from the item's first frame.  The --snr sums of a resampled item at a stream offset count its positions
+ * [snr_first, snr_last) (from its first frame) inside [0, n_emit[i]): all of them by default, a window's owned part for
+ * awm_embed_window_rates. */
 int
 embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, size_t n_values, const awm_batch_item *items, size_t n_items,
              const uint8_t *coded_bits, const uint64_t *zero_frames, const int *sample_rates, const uint64_t *n_emit, int mark_sample_rate,
              int frames_pad_start, double water_delta, int limiter_block44, int limiter_ms, float limiter_ceiling, double *snr_power,
-             size_t scratch_bytes, const uint32_t *key_index = nullptr)
+             size_t scratch_bytes, const uint32_t *key_index = nullptr, uint64_t snr_first = 0, uint64_t snr_last = UINT64_MAX)
 {
   RoleSet rs { ctx->roles.as<uint16_t>(), ctx->roles_fpb, ctx->roles_n_coded, false };
   if (key_index)
@@ -3066,6 +3068,11 @@ embed_batch (const char *name, awm_ctx *ctx, const void *in_v, void *out_v, int 
       R.coef_in = f.coef_in;
       R.coef_out = f.coef_out;
       R.limiter_block = block_of (rate);
+      {
+        const long long z = zero_frames ? (long long) zero_frames[i] : 0;
+        R.snr0 = z + (long long) std::min<uint64_t> (snr_first, n_emit[i]);
+        R.snr1 = z + (long long) std::min<uint64_t> (snr_last, n_emit[i]);
+      }
       if (zero_frames && zero_frames[i])
         {
           /* the stream of this item ends at z + n_emit, its x44 at n44 of that.  Everything before the first input frame the
@@ -3258,6 +3265,56 @@ awm_embed_batch_keys (awm_ctx *ctx, const void *in_v, void *out_v, int is_s16, s
   return embed_batch ("awm_embed_batch_keys", ctx, in_v, out_v, is_s16, n_values, items, n_items, coded_bits, zero_frames, sample_rates, n_emit,
                       mark_sample_rate, frames_pad_start, water_delta, int ((long long) mark_sample_rate * limiter_ms / 1000), limiter_ms, limiter_ceiling,
                       snr_power, scratch_bytes, key_index);
+}
+
+int
+awm_embed_window_rates (awm_ctx *ctx, const float *in, float *out, size_t n_frames, int channels, const uint8_t *coded_bits, int sample_rate,
+                        int mark_sample_rate, uint64_t stream_first, uint64_t n_emit, int frames_pad_start, double water_delta, int limiter_ms,
+                        float limiter_ceiling, uint64_t snr_first, uint64_t snr_last, double *snr_power)
+{
+  if (sample_rate == mark_sample_rate)
+    return fail (ctx, "awm_embed_window_rates: the input is at the watermark rate %d Hz (use awm_embed_window)", mark_sample_rate);
+  if (snr_first > snr_last)
+    return fail (ctx, "awm_embed_window_rates: --snr range [%llu, %llu) is reversed", (unsigned long long) snr_first, (unsigned long long) snr_last);
+  if (channels <= 0 || n_frames > AWM_MAX_STREAM_FRAMES)
+    return fail (ctx, "awm_embed_window_rates: channels %d must be > 0 and n_frames %zu at most 2^48", channels, n_frames);
+  const awm_batch_item item = { 0, n_frames, channels };
+  const size_t n_values = n_frames * size_t (channels);
+  char why[240];
+  if (awm_batch_rates_offsets_validate (&item, 1, n_values, &sample_rate, &n_emit, &stream_first, mark_sample_rate, why, sizeof (why)))
+    return fail (ctx, "awm_embed_window_rates: %s", why);
+  return embed_batch ("awm_embed_window_rates", ctx, in, out, 0, n_values, &item, 1, coded_bits, &stream_first, &sample_rate, &n_emit, mark_sample_rate,
+                      frames_pad_start, water_delta, int ((long long) mark_sample_rate * limiter_ms / 1000), limiter_ms, limiter_ceiling, snr_power, 0,
+                      nullptr, snr_first, snr_last);
+}
+
+int
+awm_window_range_rates (uint64_t own_first, uint64_t own_end, uint64_t n_total, int sample_rate, int mark_sample_rate, int limiter_ms, int hlen,
+                        uint64_t *ext_first, uint64_t *ext_end)
+{
+  if (sample_rate <= 0 || mark_sample_rate <= 0 || !resample_ratio_ok (double (mark_sample_rate) / sample_rate) ||
+      !resample_ratio_ok (double (sample_rate) / mark_sample_rate) || hlen < 8 || hlen > 96 || limiter_ms <= 0 || own_first >= own_end ||
+      own_end > n_total || own_end > AWM_MAX_STREAM_FRAMES)
+    return 1;
+  const uint64_t N = kFrame, far = AWM_MAX_STREAM_FRAMES * 64;   // "no end": beyond every stream at either rate
+  const uint64_t L = std::max<uint64_t> (uint64_t (sample_rate) * uint64_t (limiter_ms) / 1000, 1);
+  /* 1. the limiter gain of an owned frame reads the peaks of its own block and of the blocks before and after it */
+  const uint64_t b0 = own_first / L, b1 = (own_end - 1) / L;
+  const uint64_t m0 = b0 ? (b0 - 1) * L : 0, m1 = (b1 + 2) * L;
+  /* 2. every frame of those blocks reads the watermark at the watermark rate through the out-resampler's taps */
+  uint64_t w0, w1;
+  awm_resample_taps (far, double (sample_rate) / mark_sample_rate, hlen, m0, m1 - m0, &w0, &w1);
+  /* 3. a watermark sample reads the 1024-frames before and after its own (the synthesis window) */
+  const uint64_t x0 = (w0 / N ? w0 / N - 1 : 0) * N, x1 = ((std::max (w1, w0 + 1) - 1) / N + 2) * N;
+  /* 4. those frames read the input through the in-resampler's taps */
+  uint64_t e0, e1;
+  awm_resample_taps (far, double (mark_sample_rate) / sample_rate, hlen, x0, x1 - x0, &e0, &e1);
+  /* 5. one frame of margin on each side (the float positions of the taps are rounded), 6. inside the stream */
+  e0 = std::min (e0, m0);
+  e1 = std::max (e1, m1);
+  *ext_first = e0 ? e0 - 1 : 0;
+  *ext_end = std::min (e1 + 1, n_total);
+  return 0;
 }
 
 /* ---------------------------------------------------------------- speed scan */

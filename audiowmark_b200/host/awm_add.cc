@@ -332,36 +332,103 @@ window_range (size_t own_start, size_t own_end, size_t n_total, size_t limiter_b
     }
 }
 
-/* add_stream_watermark's loop (src/wmadd.cc:504-589) with bounded memory: the stream is embedded window by window.  A window
- * is run through awm_embed with the halo window_range() asks for and with first_frame_number = its position in the stream, so the
- * table row of every frame and the limiter blocks are those of a run over the whole stream and the owned part of the result
- * is bit identical to it (tests/test_gpu_sharding.py checks exactly this property for sharded embedding).  Reads block only
- * until one window + about two seconds of look-ahead are buffered: a pipe gets its first output after ~100 s of input, not at EOF.
+int
+add_window_range (size_t own_first, size_t own_end, size_t n_total, int sample_rate, size_t& ext_first, size_t& ext_end)
+{
+  if (own_first >= own_end || own_end > n_total)
+    {
+      error ("audiowmark: owned range [%zu, %zu) is empty or ends past the %zu frames of the stream\n", own_first, own_end, n_total);
+      return 1;
+    }
+  if (sample_rate == Params::mark_sample_rate)
+    {
+      window_range (own_first, own_end, n_total, size_t (sample_rate) * size_t (Params::limiter_block_size_ms) / 1000, ext_first, ext_end);
+      return 0;
+    }
+  uint64_t e0 = 0, e1 = 0;
+  if (awm_window_range_rates (own_first, own_end, n_total, sample_rate, Params::mark_sample_rate, int (Params::limiter_block_size_ms), 16, &e0, &e1))
+    {
+      error ("audiowmark: sample rate %d is outside the resampler's range\n", sample_rate);
+      return 1;
+    }
+  ext_first = e0;
+  ext_end = e1;
+  return 0;
+}
+
+int
+add_watermark_window (const Key& key, const string& bits, const float *in, float *out, size_t ext_first, size_t ext_end, size_t n_total,
+                      int n_channels, int sample_rate, size_t own_first, size_t own_end, double *snr_power)
+{
+  const vector<int> bitvec = parse_payload (bits);
+  if (bitvec.empty())
+    return 1;
+  awm_ctx *ctx = Engine::ctx();
+  if (!ctx)
+    return 1;
+  const int mark = Params::mark_sample_rate;
+  /* the --snr sums count the watermark signal before the limiter over the owned frames; a window that ends the stream also takes the
+   * frames the add loop emits after the end of the input */
+  const uint64_t snr_first = own_first - ext_first, snr_last = own_end >= n_total ? ~uint64_t (0) : own_end - ext_first;
+  int rc;
+  if (sample_rate == mark)
+    {
+      if (!Engine::set_embed_tables (key, bitvec))
+        return 1;
+      const int limiter_block = Params::test_no_limiter ? 0 : sample_rate * int (Params::limiter_block_size_ms) / 1000;
+      rc = awm_embed_window (ctx, in, out, ext_end - ext_first, n_channels, ext_first / Params::frame_size, Params::frames_pad_start, Params::water_delta,
+                             limiter_block, Params::limiter_ceiling, snr_first, snr_last, snr_power);
+    }
+  else
+    {
+      if (!Engine::set_embed_roles (key))
+        return 1;
+      /* a window that ends the stream emits what the whole stream's add loop emits after its first frame */
+      uint64_t n_emit = ext_end - ext_first;
+      if (ext_end >= n_total)
+        {
+          size_t emit = 0, runs = 0;
+          resampled_add_plan (n_total, sample_rate, !Params::test_no_limiter, size_t (sample_rate) * size_t (Params::limiter_block_size_ms) / 1000, emit, runs);
+          n_emit = std::max (emit, n_total) - ext_first;
+        }
+      const vector<uint8_t> coded = gen_coded_bits (key, bitvec);
+      rc = awm_embed_window_rates (ctx, in, out, ext_end - ext_first, n_channels, coded.data(), sample_rate, mark, ext_first, n_emit,
+                                   Params::frames_pad_start, Params::water_delta, Params::test_no_limiter ? 0 : int (Params::limiter_block_size_ms),
+                                   Params::limiter_ceiling, snr_first, snr_last, snr_power);
+    }
+  if (rc)
+    {
+      error ("audiowmark: embedding failed: %s\n", awm_last_error (ctx));
+      return 1;
+    }
+  return 0;
+}
+
+/* add_stream_watermark's loop (src/wmadd.cc:504-589) with bounded memory: the stream is embedded window by window through
+ * add_watermark_window, each window with the halo add_window_range asks for, so the owned part of every window is bit identical
+ * to a run over the whole stream.  Reads block only until one window and its look-ahead (about two limiter blocks) are buffered:
+ * a pipe gets its first output after ~100 s of input, not at EOF.
  * zero_frames: the input continues a stream that began zero_frames earlier with silence (HLS segments, src/wmadd.cc:504-519):
- * positions, table rows and limiter blocks count from there, nothing is written for the silent part.
- * window_frames = 0: default window (4096 1024-frames = 95 s); tests pass small windows. */
+ * positions, table rows, resamplers and limiter blocks count from there, nothing is written for the silent part.
+ * window_frames = 0: default window (4096 1024-frames = 95 s at 44.1 kHz); tests pass small windows. */
 int
 add_watermark_windowed (const Key& key, const std::function<Error (vector<float>&, size_t)>& read, const std::function<Error (const vector<float>&)>& write,
                         int n_channels, int sample_rate, const string& bits, size_t zero_frames, size_t window_frames, AddStats *stats, size_t *frames_written)
 {
   const size_t N = Params::frame_size, C = size_t (n_channels);
-  const size_t L = size_t (sample_rate) * size_t (Params::limiter_block_size_ms) / 1000;      // limiter block; also sizes the halo without limiter
+  const size_t L = size_t (sample_rate) * size_t (Params::limiter_block_size_ms) / 1000;
   const size_t W = (window_frames ? window_frames : 4096) * N;
   const size_t unknown = ~size_t (0);
-  const vector<int> bitvec = parse_payload (bits);
-  if (bitvec.empty())
+  if (parse_payload (bits).empty())
     return 1;
-  awm_ctx *ctx = Engine::ctx();
-  if (!ctx || !Engine::set_embed_tables (key, bitvec))
-    return 1;
-  const int limiter_block = Params::test_no_limiter ? 0 : int (L);
   vector<float> pending;                         // stream positions [p0, p1), interleaved
   size_t p0 = 0, p1 = 0, own_start = zero_frames, written = 0;
   double snr_delta = 0, snr_signal = 0;
   {
     /* the silent prefix is never materialised beyond what the first window's halo reaches into */
     size_t e0, e1;
-    window_range (own_start, own_start + 1, unknown, L, e0, e1);
+    if (add_window_range (own_start, own_start + 1, unknown, sample_rate, e0, e1))
+      return 1;
     p0 = e0;
     p1 = zero_frames;
     pending.assign ((p1 - p0) * C, 0.f);
@@ -371,7 +438,8 @@ add_watermark_windowed (const Key& key, const std::function<Error (vector<float>
   while (!eof || own_start < p1)
     {
       size_t e0, e1;
-      window_range (own_start, own_start + W, unknown, L, e0, e1);
+      if (add_window_range (own_start, own_start + W, unknown, sample_rate, e0, e1))
+        return 1;
       while (!eof && p1 < e1)                    // the window and its look-ahead
         {
           const Error err = read (block, std::min<size_t> (e1 - p1, 1 << 16));
@@ -389,17 +457,13 @@ add_watermark_windowed (const Key& key, const std::function<Error (vector<float>
       const size_t own_end = eof ? p1 : own_start + W;
       if (own_end <= own_start)
         break;
-      window_range (own_start, own_end, n_total, L, e0, e1);
+      if (add_window_range (own_start, own_end, n_total, sample_rate, e0, e1))
+        return 1;
       out.resize ((e1 - e0) * C);
       double snr_power[2] = { 0, 0 };
-      /* the --snr sums count the watermark signal before the limiter, over this window's own part (the last window also takes the
-       * zero padded frames after the end of the input, like the reference loop) */
-      if (awm_embed_window (ctx, pending.data() + (e0 - p0) * C, out.data(), e1 - e0, n_channels, e0 / N, Params::frames_pad_start, Params::water_delta,
-                            limiter_block, Params::limiter_ceiling, own_start - e0, eof ? ~uint64_t (0) : own_end - e0, (Params::snr || stats) ? snr_power : nullptr))
-        {
-          error ("audiowmark: embedding failed: %s\n", awm_last_error (ctx));
-          return 1;
-        }
+      if (add_watermark_window (key, bits, pending.data() + (e0 - p0) * C, out.data(), e0, e1, n_total, n_channels, sample_rate, own_start, own_end,
+                                (Params::snr || stats) ? snr_power : nullptr))
+        return 1;
       snr_delta += snr_power[0];
       snr_signal += snr_power[1];
       const float *o = out.data() + (own_start - e0) * C;
@@ -413,14 +477,20 @@ add_watermark_windowed (const Key& key, const std::function<Error (vector<float>
       own_start = own_end;
       if (eof)
         break;
-      window_range (own_start, own_start + 1, unknown, L, e0, e1);   // what the next window still needs of the buffer
+      if (add_window_range (own_start, own_start + 1, unknown, sample_rate, e0, e1))   // what the next window still needs of the buffer
+        return 1;
       pending.erase (pending.begin(), pending.begin() + (e0 - p0) * C);
       p0 = e0;
     }
   if (frames_written)
     *frames_written = written;
   if (stats)
-    *stats = add_stats (gen_runs (p1, !Params::test_no_limiter, L), snr_delta, snr_signal);
+    {
+      size_t emit = 0, runs = gen_runs (p1, !Params::test_no_limiter, L);
+      if (sample_rate != Params::mark_sample_rate)
+        resampled_add_plan (p1, sample_rate, !Params::test_no_limiter, L, emit, runs);
+      *stats = add_stats (runs, snr_delta, snr_signal);
+    }
   return 0;
 }
 
@@ -455,40 +525,10 @@ add_stream_watermark (const Key& key, AudioInputStream *in_stream, AudioOutputSt
   AddStats stats;
   size_t total_output_frames = 0;
   Error err;
-  if (in_stream->sample_rate() != Params::mark_sample_rate)
-    {
-      /* other sample rates go through the resamplers around the embedder (a one-item awm_embed_batch_rates): whole stream at once */
-      if (zero_frames)
-        {
-          error ("audiowmark: stream offsets are only supported at %d Hz\n", Params::mark_sample_rate);
-          return 1;
-        }
-      WavData wav;
-      err = wav.load (in_stream);
-      if (err)
-        {
-          error ("audiowmark: input stream read failed: %s\n", err.message());
-          return 1;
-        }
-      vector<float> out (wav.n_values());
-      if (add_watermark_buffer (key, wav.samples().data(), out.data(), wav.n_frames(), wav.n_channels(), wav.sample_rate(), bits, &stats))
-        return 1;
-      vector<float>().swap (wav.mutable_samples());
-      err = out_stream->write_frames (out);
-      if (err)
-        {
-          error ("audiowmark output write failed: %s\n", err.message());
-          return 1;
-        }
-      total_output_frames = out.size() / std::max (in_stream->n_channels(), 1);
-    }
-  else
-    {
-      auto read = [&] (vector<float>& samples, size_t count) { return in_stream->read_frames (samples, count); };
-      auto write = [&] (const vector<float>& samples) { return out_stream->write_frames (samples); };
-      if (add_watermark_windowed (key, read, write, in_stream->n_channels(), in_stream->sample_rate(), bits, zero_frames, 0, &stats, &total_output_frames))
-        return 1;
-    }
+  auto read = [&] (vector<float>& samples, size_t count) { return in_stream->read_frames (samples, count); };
+  auto write = [&] (const vector<float>& samples) { return out_stream->write_frames (samples); };
+  if (add_watermark_windowed (key, read, write, in_stream->n_channels(), in_stream->sample_rate(), bits, zero_frames, 0, &stats, &total_output_frames))
+    return 1;
   if (Params::snr)
     info ("SNR:          %f dB\n", stats.snr_db);
   info ("Data Blocks:  %d\n", stats.data_blocks);

@@ -367,6 +367,40 @@ awmh_add_windowed (const unsigned char *key16, const float *in, float *out, size
   return written == n_frames ? 0 : -3;
 }
 
+/* add_window_range: the input frames a window needs for its owned frames (n_total = UINT64_MAX: the end is not known yet) */
+int
+awmh_window_range (uint64_t own_first, uint64_t own_end, uint64_t n_total, int sample_rate, uint64_t *ext_first, uint64_t *ext_end)
+{
+  size_t e0 = 0, e1 = 0;
+  if (add_window_range (own_first, own_end, n_total, sample_rate, e0, e1))
+    return 2;
+  *ext_first = e0;
+  *ext_end = e1;
+  return 0;
+}
+
+/* add_watermark_window on a buffer (host or device) that holds stream frames [stream_first, stream_first + n_frames): the window
+ * add_window_range names for [own_first, own_end) is embedded in place of the same frames of `out`, the rest of `out` is not
+ * touched.  snr_power (optional): the --snr sums of the owned frames.  Returns 2, before any GPU work, for a malformed range or a
+ * buffer that misses a frame of the window, 1 for other errors. */
+int
+awmh_add_window (const unsigned char *key16, const float *in, float *out, uint64_t stream_first, size_t n_frames, int n_channels, int sample_rate,
+                 const char *payload_hex, uint64_t n_total, uint64_t own_first, uint64_t own_end, double *snr_power)
+{
+  size_t e0 = 0, e1 = 0;
+  if (n_channels <= 0 || add_window_range (own_first, own_end, n_total, sample_rate, e0, e1))
+    return 2;
+  if (e0 < stream_first || e1 > stream_first + n_frames)
+    {
+      error ("audiowmark: the buffer holds stream frames [%llu, %llu), the window needs [%zu, %zu)\n", (unsigned long long) stream_first,
+             (unsigned long long) (stream_first + n_frames), e0, e1);
+      return 2;
+    }
+  const size_t off = (e0 - stream_first) * size_t (n_channels);
+  return add_watermark_window (make_key (key16, ""), payload_hex, in + off, out + off, e0, e1, n_total, n_channels, sample_rate, own_first, own_end,
+                               snr_power);
+}
+
 static int result_json (ResultSet& result_set, size_t mark_rate_frames, char *json_out, size_t json_cap, int *n_patterns);
 
 int

@@ -41,6 +41,17 @@ int add_watermark_windowed (const Key& key, const std::function<Error (std::vect
                             const std::function<Error (const std::vector<float>&)>& write, int n_channels, int sample_rate, const std::string& bits,
                             size_t zero_frames, size_t window_frames, AddStats *stats, size_t *frames_written);
 
+/* The input frames [ext_first, ext_end) a window needs so that its owned frames [own_first, own_end) come out as in a run over the
+ * whole stream of n_total frames (~0: not known yet): window_range at 44.1 kHz (ext_first a multiple of 1024, as awm_embed_window
+ * needs), awm_window_range_rates at other rates.  Returns 1, with a message, for a bad range or rate. */
+int add_window_range (size_t own_first, size_t own_end, size_t n_total, int sample_rate, size_t& ext_first, size_t& ext_end);
+/* One window of a stream at any rate: in / out hold stream frames [ext_first, ext_end), the range add_window_range names for the
+ * owned frames [own_first, own_end) of a stream of n_total frames (~0: not known yet, so the window does not end it).  The owned
+ * frames of out come out bit identical to add_watermark_buffer of the whole stream.  snr_power (optional, 2 doubles) receives the
+ * --snr sums of the owned frames; the window that ends the stream also takes the frames the add loop emits after the input. */
+int add_watermark_window (const Key& key, const std::string& bits, const float *in, float *out, size_t ext_first, size_t ext_end, size_t n_total,
+                          int n_channels, int sample_rate, size_t own_first, size_t own_end, double *snr_power);
+
 /* frame counts of the add loop for inputs that are not at the watermark rate (see awm_add.cc) */
 void resampled_add_plan (size_t n_frames, int sample_rate, bool limiter_on, size_t limiter_block, size_t& n_emit, size_t& gen_runs_out);
 

@@ -17,7 +17,8 @@ CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
            "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_bg_input_range", "awmh_add_windowed",
-           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_role_layout", "awmh_embed_roles_device"]
+           "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_role_layout", "awmh_embed_roles_device",
+           "awmh_window_range", "awmh_add_window"]
 
 _lib = None
 
@@ -328,7 +329,9 @@ def add_batch_rates(pcms, payloads, sample_rates, key=None, items=None, out=None
 
 
 def add_windowed(pcm_in: np.ndarray, payload_hex: str, key=None, zero_frames=0, window_frames=0, sample_rate=44100):
-    """the bounded-memory loop of `audiowmark add` (add_watermark_windowed) on a host buffer -> (output, data blocks, snr dB)"""
+    """the bounded-memory loop of `audiowmark add` (add_watermark_windowed) on a host buffer -> (output, data blocks, snr dB), at any
+    sample rate: the output equals add(zeros(zero_frames) ++ pcm_in, sample_rate=sample_rate)[zero_frames:] bit for bit.  window_frames
+    (in 1024-frames; 0: the default of 4096) sets how much is marked per window."""
     pcm_in = np.ascontiguousarray(pcm_in, np.float32)
     out = np.empty_like(pcm_in)
     blocks, snr = ctypes.c_int(), ctypes.c_double()
@@ -337,6 +340,47 @@ def add_windowed(pcm_in: np.ndarray, payload_hex: str, key=None, zero_frames=0, 
     if rc:
         raise RuntimeError("awmh_add_windowed failed (rc=%d); see stderr" % rc)
     return out, blocks.value, snr.value
+
+
+UNKNOWN = (1 << 64) - 1        # n_total of a stream whose end is not known yet
+
+
+def window_range(own_first: int, own_end: int, n_total: int, sample_rate=44100) -> tuple[int, int]:
+    """the input frames [ext_first, ext_end) that add_window needs so that its owned frames [own_first, own_end) come out as in add()
+    of the whole stream of n_total frames (UNKNOWN: the end is not known yet).  At 44.1 kHz ext_first is a multiple of 1024; at other
+    rates it is the smallest such range (awm_window_range_rates).  ValueError for an empty range, one past n_total or a bad rate."""
+    first, end = ctypes.c_uint64(), ctypes.c_uint64()
+    rc = load().awmh_window_range(ctypes.c_uint64(own_first), ctypes.c_uint64(own_end), ctypes.c_uint64(n_total), ctypes.c_int(sample_rate),
+                                  ctypes.byref(first), ctypes.byref(end))
+    if rc:
+        raise ValueError("window_range: owned range [%d, %d) of %d frames at %d Hz is refused; see stderr" % (own_first, own_end, n_total, sample_rate))
+    return first.value, end.value
+
+
+def add_window(pcm, payload_hex: str, stream_first: int, n_total: int, own_first: int, own_end: int, key=None, pcm_out=None, n_frames=None,
+               channels=None, sample_rate=44100, want_stats=False):
+    """`add` of one window of a stream at any rate: how a rank marks its own span of a master.  pcm holds stream frames
+    [stream_first, stream_first + n_frames) (a numpy array [n, channels], or a device pointer with n_frames / channels and pcm_out)
+    and must cover window_range(own_first, own_end, n_total, sample_rate); n_total may be UNKNOWN for a window that does not end the
+    stream.  The window's frames of pcm_out are written (a numpy result starts as a copy of pcm), and its owned frames [own_first,
+    own_end) equal those of add() of the whole stream bit for bit.  want_stats: also the --snr sums (watermark power, signal power) of
+    the owned frames (the window that ends the stream includes the frames emitted after it); summed over all windows,
+    10 log10 (signal / watermark) is the stream's SNR.  ValueError when the buffer misses part of the window or the range is bad."""
+    if isinstance(pcm, np.ndarray):
+        pcm = np.ascontiguousarray(pcm, np.float32)
+        n_frames, channels = pcm.shape
+        if pcm_out is None:
+            pcm_out = pcm.copy()
+    snr = np.zeros(2, np.float64)
+    rc = load().awmh_add_window(_key(key), _ptr(pcm), _ptr(pcm_out), ctypes.c_uint64(stream_first), ctypes.c_size_t(n_frames), ctypes.c_int(channels),
+                                ctypes.c_int(sample_rate), payload_hex.encode(), ctypes.c_uint64(n_total), ctypes.c_uint64(own_first),
+                                ctypes.c_uint64(own_end), _ptr(snr) if want_stats else None)
+    if rc == 2:
+        raise ValueError("add_window: buffer [%d, +%d) at %d Hz does not cover the window of [%d, %d), or the range is bad; see stderr"
+                         % (stream_first, n_frames, sample_rate, own_first, own_end))
+    if rc:
+        raise RuntimeError("awmh_add_window failed (rc=%d); see stderr" % rc)
+    return (pcm_out, float(snr[0]), float(snr[1])) if want_stats else pcm_out
 
 
 def get(pcm, keys=None, names=None, n_frames=None, channels=None, sample_rate=44100, parse=True):

@@ -47,7 +47,8 @@ def assign_chunks(n_chunks: int, world: int):
 
 def embed_range(own_start: int, own_end: int, n_frames: int, limiter_block: int):
     """Extended range [ext_start, ext_end) a rank has to embed so that [own_start, own_end) comes out exactly as in the
-    unsharded run.  ext_start is a multiple of 1024 (-> first_frame_number); returns (ext_start, ext_end, first_frame_number)."""
+    unsharded run.  ext_start is a multiple of 1024 (-> first_frame_number); returns (ext_start, ext_end, first_frame_number).
+    44.1 kHz only: at any sample rate a rank takes its range from hostapi.window_range and marks it with hostapi.add_window."""
     if own_start <= 0:
         ext_start = 0
     else:

@@ -255,6 +255,28 @@ int awm_embed_batch_rates_offsets (awm_ctx *ctx, const void *in, void *out, int 
                                    int mark_sample_rate, int frames_pad_start, double water_delta, int limiter_ms, float limiter_ceiling,
                                    double *snr_power, size_t scratch_bytes);
 
+/* awm_embed_window for input that is not at mark_sample_rate (streaming and sharded `add` of a 48 kHz master): in / out hold stream
+ * frames [stream_first, stream_first + n_frames) (interleaved float, host or device, any 4-byte alignment) and come out exactly as
+ * item 0 of awm_embed_batch_rates_offsets with zero_frames = stream_first and this n_emit: the stream is taken as silent before the
+ * window.  n_emit counts from stream_first: the window's own length for a window that does not end the stream, the whole stream's
+ * n_emit (resampled_add_plan) minus stream_first for the last one.  A window with the halo awm_window_range_rates names for its owned
+ * frames reproduces those frames of the whole stream's `add` bit for bit.  Roles come from awm_set_embed_roles, coded_bits is uint8
+ * [2 (A, B)][n_coded_bits] as for the batched calls.  Only buffer positions [snr_first, snr_last) (inside [0, n_emit)) enter the
+ * --snr sums.  Refused before any work: sample_rate == mark_sample_rate (use awm_embed_window), snr_first > snr_last, and whatever
+ * awm_batch_rates_offsets_validate refuses for this one item (n_emit < n_frames among it). */
+int awm_embed_window_rates (awm_ctx *ctx, const float *in, float *out, size_t n_frames, int channels, const uint8_t *coded_bits, int sample_rate,
+                            int mark_sample_rate, uint64_t stream_first, uint64_t n_emit, int frames_pad_start, double water_delta, int limiter_ms,
+                            float limiter_ceiling, uint64_t snr_first, uint64_t snr_last, double *snr_power);
+/* The smallest input range [*ext_first, *ext_end) of a stream at sample_rate that makes outputs [own_first, own_end) of
+ * awm_embed_window_rates exact: the limiter blocks before, of and after the owned frames (block sample_rate * limiter_ms / 1000,
+ * which sizes the halo even when the embed runs without limiter), the out-resampler's taps into the watermark, one 1024-frame of
+ * synthesis window on each side, the in-resampler's taps into the input, one frame of margin, clamped to [0, n_total).
+ * n_total = UINT64_MAX: the end of the stream is not known yet.  Any cut is valid, no alignment is needed.  Returns nonzero, and
+ * sets nothing, for an empty owned range, one that ends past n_total or 2^48, a rate outside the resampler's range, hlen outside
+ * [8, 96] or limiter_ms <= 0.  Needs no device. */
+int awm_window_range_rates (uint64_t own_first, uint64_t own_end, uint64_t n_total, int sample_rate, int mark_sample_rate, int limiter_ms, int hlen,
+                            uint64_t *ext_first, uint64_t *ext_end);
+
 /* ---- batched embed with a key per item ----------------------------------------------------------------------------------
  * What the role table of a key (gen_embed_roles on the host: UpDownGen, BitPosGen and gen_mix_entries, src/wmcommon.cc:143-202)
  * depends on besides the key: the frame counts of one block, frames_per_bit, --linear and the code length. */
