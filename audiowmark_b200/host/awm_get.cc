@@ -437,7 +437,7 @@ struct PcmRef
  * approx_slot >= 0: one key, no speed detection; the chunk's approx search has been queued into that slot (awm_sync_approx_enqueue) */
 int
 decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vector<Key>& key_list, const PcmRef& pcm, size_t n_frames,
-              int n_channels, int sample_rate, bool first_chunk, bool print_speed_results = false, int approx_slot = -1)
+              int n_channels, int sample_rate, bool first_chunk, bool print_speed_results, int approx_slot)
 {
   awm_ctx *ctx = Engine::ctx();
   if (!ctx)
@@ -524,29 +524,6 @@ decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vect
 } // namespace get_detail
 
 using namespace get_detail;
-
-/* BlockDecoder job list of one chunk as flat records (for the multi-GPU driver):
- * u8 code_type (AWM_BLOCK_*), u8 pattern_type (ResultSet::Type), u8 score_block_type, u8 pad, f64 time, u64 index, f64 quality, u32 n_soft, f32 soft[] */
-std::vector<unsigned char>
-block_jobs_blob (const Key& key, const vector<SyncFinder::Score>& sync_scores, const vector<vector<float>>& raw, const vector<int>& valid, int sample_rate, int *n_jobs)
-{
-  vector<VitJob> jobs;
-  build_block_jobs (key, sync_scores, raw, valid, sample_rate, 0, 1, jobs);
-  std::vector<unsigned char> b;
-  auto put = [&] (const void *p, size_t n) { const unsigned char *c = static_cast<const unsigned char *> (p); b.insert (b.end(), c, c + n); };
-  for (const auto& j : jobs)
-    {
-      const uint8_t hdr[4] = { uint8_t (j.block_type == ConvBlockType::a ? AWM_BLOCK_A : j.block_type == ConvBlockType::b ? AWM_BLOCK_B : AWM_BLOCK_AB),
-                               uint8_t (j.type), uint8_t (j.score.block_type), 0 };
-      const double time = j.time, quality = j.score.quality;
-      const uint64_t index = j.score.index;
-      const uint32_t n_soft = j.soft.size();
-      put (hdr, 4); put (&time, 8); put (&index, 8); put (&quality, 8); put (&n_soft, 4);
-      put (j.soft.data(), n_soft * sizeof (float));
-    }
-  *n_jobs = int (jobs.size());
-  return b;
-}
 
 /* chunk geometry of WavChunkLoader (src/wavchunkloader.cc:54-163): chunks of get_chunk_size minutes that
  * overlap by two blocks * 1.3 */
@@ -688,29 +665,6 @@ get_watermark_pcm (const vector<Key>& key_list, const float *samples, const int1
       result_set.merge (chunk_results[c]);
     }
   result_set.sort (key_list);
-  return 0;
-}
-
-int
-get_watermark_chunk (const vector<Key>& key_list, const float *samples, size_t n_frames, int n_channels, int sample_rate,
-                     bool first_chunk, ResultSet& chunk_result)
-{
-  if (sample_rate != Params::mark_sample_rate)
-    {
-      error ("audiowmark: input sample rate %d: only %d Hz is supported\n", sample_rate, Params::mark_sample_rate);
-      return 1;
-    }
-  vector<VitJob> pending;
-  string debug_sync;
-  PcmRef pcm;
-  pcm.f32 = samples;
-  if (decode_chunk (pending, 0, debug_sync, key_list, pcm, n_frames, n_channels, sample_rate, first_chunk))
-    return 1;
-  vector<ResultSet> one (1);
-  if (!run_viterbi_jobs (pending, one))
-    return 1;
-  one[0].set_debug_sync (debug_sync);
-  chunk_result.merge (one[0]);
   return 0;
 }
 

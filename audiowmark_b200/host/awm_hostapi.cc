@@ -21,9 +21,6 @@ make_key (const unsigned char *key16, const char *name)
   return k;
 }
 
-std::vector<unsigned char> block_jobs_blob (const Key& key, const std::vector<SyncFinder::Score>& sync_scores, const std::vector<std::vector<float>>& raw,
-                                            const std::vector<int>& valid, int sample_rate, int *n_jobs);
-
 extern "C" {
 
 void
@@ -458,40 +455,11 @@ result_json (ResultSet& result_set, size_t mark_rate_frames, char *json_out, siz
   return 0;
 }
 
-/* ---- sharded `get`: chunk results as flat records ------------------------------------------------
- * record (little endian, packed): i32 key_index, f64 time, f64 quality, u64 sync_index, f32 decode_error,
- * u8 block_type, u8 type, f64 speed, u16 n_bits, n_bits bytes (0/1)
+/* ---- test aid (CPU): ResultSet merge, sort and --json print of per-chunk pattern records ----------------------
+ * awmh_merge_chunks takes the chunk results as the test writes them, so that the C++ ResultSet can be checked against the oracle's
+ * without a GPU, printed digits included.  Record (little endian, packed): i32 key_index, f64 time, f64 quality, u64 sync_index,
+ * f32 decode_error, u8 block_type, u8 type, f64 speed, u16 n_bits, n_bits bytes (0/1)
  */
-static void
-put (std::vector<unsigned char>& b, const void *p, size_t n)
-{
-  const unsigned char *c = static_cast<const unsigned char *> (p);
-  b.insert (b.end(), c, c + n);
-}
-
-static std::vector<unsigned char>
-serialize (const ResultSet& rs, const std::vector<Key>& key_list)
-{
-  std::vector<unsigned char> b;
-  for (const auto& p : rs.all())
-    {
-      int32_t ki = 0;
-      for (size_t k = 0; k < key_list.size(); k++)
-        if (key_list[k] == p.key)
-          ki = k;
-      const double time = p.time, quality = p.sync_score.quality, speed = p.speed;
-      const uint64_t idx = p.sync_score.index;
-      const float err = p.decode_error;
-      const uint8_t bt = uint8_t (p.sync_score.block_type), ty = uint8_t (p.type);
-      const uint16_t nb = p.bit_vec.size();
-      put (b, &ki, 4); put (b, &time, 8); put (b, &quality, 8); put (b, &idx, 8); put (b, &err, 4);
-      put (b, &bt, 1); put (b, &ty, 1); put (b, &speed, 8); put (b, &nb, 2);
-      for (int bit : p.bit_vec)
-        b.push_back (bit ? 1 : 0);
-    }
-  return b;
-}
-
 static bool
 deserialize (const unsigned char *b, size_t len, const std::vector<Key>& key_list, ResultSet& rs)
 {
@@ -519,26 +487,7 @@ make_key_list (const unsigned char *keys16, const char *const *names, int n_keys
   return key_list;
 }
 
-/* decode ONE chunk of the reference's chunk geometry (pcm = the chunk's samples); records -> blob_out */
-int
-awmh_get_chunk (const unsigned char *keys16, const char *const *names, int n_keys, const float *pcm, size_t n_frames, int n_channels,
-                int sample_rate, int first_chunk, unsigned char *blob_out, size_t blob_cap, size_t *blob_len)
-{
-  const std::vector<Key> key_list = make_key_list (keys16, names, n_keys);
-  ResultSet rs;
-  const int rc = get_watermark_chunk (key_list, pcm, n_frames, n_channels, sample_rate, first_chunk != 0, rs);
-  if (rc)
-    return rc;
-  const std::vector<unsigned char> b = serialize (rs, key_list);
-  *blob_len = b.size();
-  if (b.size() > blob_cap)
-    return -2;
-  if (!b.empty())
-    memcpy (blob_out, b.data(), b.size());
-  return 0;
-}
-
-/* ResultSet::merge in chunk order + sort + --json document (src/wmget.cc:289-316,252-287,340-382) from chunk blobs */
+/* ResultSet::merge in chunk order + sort + --json document (src/wmget.cc:289-316,252-287,340-382) from chunk records */
 int
 awmh_merge_chunks (const unsigned char *keys16, const char *const *names, int n_keys, const unsigned char *const *blobs, const size_t *blob_lens,
                    const double *time_offsets, int n_chunks, double total_seconds, char *json_out, size_t json_cap)
@@ -790,7 +739,7 @@ awmh_bg_input_range (uint64_t n_total, int rank, int world, int sample_rate, uin
   return 0;
 }
 
-/* ---- stage-level access for the frame-balanced multi-GPU driver (audiowmark_b200/sharding.py) ---------------- */
+/* ---- the GPU context and its key slots ------------------------------------------------------------------------- */
 
 void *
 awmh_ctx()
@@ -935,7 +884,8 @@ awmh_sync_trace_fetch (double *rows, size_t max_rows, size_t *n_rows)
   return n <= max_rows ? 0 : -2;
 }
 
-/* candidates of one chunk from its (gathered) peak list, complete above floor_q; *complete = 0 -> ask again with a lower floor */
+/* test aid (CPU): select_candidates_from_peaks, the selection of the single-GPU and the sharded `get`, on a peak list the test builds.
+ * Candidates of one chunk from its (gathered) peak list, complete above floor_q; *complete = 0 -> ask again with a lower floor */
 int
 awmh_stage_select (const awm_search_score *peaks, size_t n, double floor_q, int clip_mode, awm_search_score *out, size_t max_out, size_t *n_out, int *complete)
 {
@@ -953,46 +903,6 @@ awmh_stage_select (const awm_search_score *peaks, size_t n, double floor_q, int 
     return -2;
   if (!sel.empty())
     memcpy (out, sel.data(), sel.size() * sizeof (awm_search_score));
-  return 0;
-}
-
-/* threshold2 / n-best selection of a chunk's refined scores -> (index, quality, block type) sorted by index */
-int
-awmh_stage_final (const awm_search_score *refined, size_t n, uint64_t *index_out, double *quality_out, int *btype_out, size_t *n_out)
-{
-  std::vector<awm_search_score> v (refined, refined + n);
-  std::vector<SyncFinder::Score> out;
-  select_final_scores (v, out);
-  *n_out = out.size();
-  for (size_t i = 0; i < out.size(); i++)
-    {
-      index_out[i] = out[i].index;
-      quality_out[i] = out[i].quality;
-      btype_out[i] = int (out[i].block_type);
-    }
-  return 0;
-}
-
-/* Viterbi job list (single blocks, AB pairs, "all") of one chunk from its final scores and their soft bits */
-int
-awmh_stage_jobs (const unsigned char *key16, const uint64_t *index, const double *quality, const int *btype, size_t n, const float *raw, const int *valid,
-                 int sample_rate, unsigned char *blob, size_t cap, size_t *len, int *n_jobs)
-{
-  const size_t n_coded = code_size (ConvBlockType::a, Params::payload_size);
-  std::vector<SyncFinder::Score> scores (n);
-  std::vector<std::vector<float>> rawv (n);
-  std::vector<int> validv (valid, valid + n);
-  for (size_t i = 0; i < n; i++)
-    {
-      scores[i] = SyncFinder::Score { size_t (index[i]), quality[i], ConvBlockType (btype[i]) };
-      rawv[i].assign (raw + i * n_coded, raw + (i + 1) * n_coded);
-    }
-  const std::vector<unsigned char> b = block_jobs_blob (make_key (key16, ""), scores, rawv, validv, sample_rate, n_jobs);
-  *len = b.size();
-  if (b.size() > cap)
-    return -2;
-  if (!b.empty())
-    memcpy (blob, b.data(), b.size());
   return 0;
 }
 

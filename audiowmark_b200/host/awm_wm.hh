@@ -67,10 +67,7 @@ int get_watermark_pcm (const std::vector<Key>& key_list, const float *samples, c
 int add_watermark_buffer_s16 (const Key& key, const int16_t *in, int16_t *out, size_t n_frames, int n_channels, int sample_rate,
                               const std::string& bits, AddStats *stats, uint64_t first_frame_number = 0);
 
-/* chunk-level pieces of get_watermark_buffer for sharded runs (one process per GPU): a rank decodes some of the
- * reference's chunks (WavChunkLoader geometry) and the chunk result sets are merged in chunk order afterwards */
-int get_watermark_chunk (const std::vector<Key>& key_list, const float *samples, size_t n_frames, int n_channels, int sample_rate,
-                         bool first_chunk, ResultSet& chunk_result);
+/* the reference's chunks (WavChunkLoader geometry), which get_watermark_buffer and the sharded `get` both walk */
 void chunk_geometry (int sample_rate, size_t& max_frames, size_t& overlap_frames);
 
 int frame_count (const WavData& wav_data);
@@ -95,8 +92,8 @@ public:
   static std::vector<TraceRecord> trace_take();
 };
 
-/* stage functions of SyncFinder::search / BlockDecoder::run, used by get_watermark_buffer and by the frame-balanced
- * multi-GPU driver (audiowmark_b200/sharding.py), which runs the GPU stages on slices of a chunk on different ranks */
+/* stage functions of SyncFinder::search / BlockDecoder::run, used by get_watermark_buffer and by the sharded `get`
+ * (host/awm_balanced.cc), which runs the GPU stages on slices of a chunk on different ranks */
 int  select_candidates_from_peaks (const awm_search_score *peaks, size_t n, double floor_q, double threshold, std::vector<awm_search_score>& out,
                                   size_t truncate_n = 0);
 void select_final_scores (std::vector<awm_search_score>& scores, std::vector<SyncFinder::Score>& out);

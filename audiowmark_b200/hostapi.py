@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libawm_host.so")
 CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
-           "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_get_chunk", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_stage_final", "awmh_stage_jobs", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_bg_input_range", "awmh_add_windowed",
+           "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_bg_input_range", "awmh_add_windowed",
            "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_role_layout", "awmh_embed_roles_device",
            "awmh_window_range", "awmh_add_window"]
 
@@ -526,27 +526,9 @@ def chunk_geometry(sample_rate=44100):
     return m.value, o.value
 
 
-def get_chunk(pcm, first_chunk: bool, keys=None, names=None, n_frames=None, channels=None, sample_rate=44100) -> bytes:
-    """decode one chunk; returns the chunk's pattern records (bytes) for merge_chunks."""
-    keys = keys or [bytes(16)]
-    names = names or [""] * len(keys)
-    if isinstance(pcm, np.ndarray):
-        pcm = np.ascontiguousarray(pcm, np.float32)
-        n_frames, channels = pcm.shape
-    kb = b"".join(_key(k) for k in keys)
-    name_arr = (ctypes.c_char_p * len(keys))(*[n.encode() for n in names])
-    cap = 1 << 20
-    buf = ctypes.create_string_buffer(cap)
-    blen = ctypes.c_size_t()
-    rc = load().awmh_get_chunk(kb, name_arr, ctypes.c_int(len(keys)), _ptr(pcm), ctypes.c_size_t(n_frames), ctypes.c_int(channels),
-                               ctypes.c_int(sample_rate), ctypes.c_int(1 if first_chunk else 0), buf, ctypes.c_size_t(cap), ctypes.byref(blen))
-    if rc:
-        raise RuntimeError("awmh_get_chunk failed (rc=%d); see stderr" % rc)
-    return ctypes.string_at(buf, blen.value)
-
-
 def merge_chunks(blobs, time_offsets, total_seconds: float, keys=None, names=None) -> dict:
-    """ResultSet::merge in chunk order + sort -> the --json document."""
+    """test aid (CPU): ResultSet::merge in chunk order + sort -> the --json document, from per-chunk pattern records (bytes in the
+    record format of host/awm_hostapi.cc) that a test writes, so that the C++ ResultSet can be checked against the oracle's."""
     keys = keys or [bytes(16)]
     names = names or [""] * len(keys)
     kb = b"".join(_key(k) for k in keys)
@@ -699,6 +681,7 @@ def key_slot(key=None) -> int:
 
 
 def stage_select(peaks: np.ndarray, floor_q: float, clip_mode=False):
+    """test aid (CPU): the candidate selection of `get` (select_candidates_from_peaks) on a peak list -> (candidates, complete)"""
     pk = np.ascontiguousarray(peaks, capi.SEARCH_SCORE)
     out = np.zeros(max(len(pk), 1), capi.SEARCH_SCORE)
     n, complete = ctypes.c_size_t(), ctypes.c_int()
@@ -707,38 +690,6 @@ def stage_select(peaks: np.ndarray, floor_q: float, clip_mode=False):
     if rc:
         raise RuntimeError("awmh_stage_select failed (%d)" % rc)
     return out[:n.value].copy(), bool(complete.value)
-
-
-def stage_final(refined: np.ndarray):
-    r = np.ascontiguousarray(refined, capi.SEARCH_SCORE)
-    idx, q, bt = np.zeros(len(r), np.uint64), np.zeros(len(r), np.float64), np.zeros(len(r), np.int32)
-    n = ctypes.c_size_t()
-    load().awmh_stage_final(_ptr(r), ctypes.c_size_t(len(r)), _ptr(idx), _ptr(q), _ptr(bt), ctypes.byref(n))
-    return idx[:n.value].copy(), q[:n.value].copy(), bt[:n.value].copy()
-
-
-def stage_jobs(key, index, quality, btype, raw, valid, sample_rate=44100):
-    """Viterbi jobs of one chunk: list of (code_type, pattern_type, score_btype, time, index, quality, soft float32[])"""
-    import struct
-    idx, q, bt = (np.ascontiguousarray(index, np.uint64), np.ascontiguousarray(quality, np.float64), np.ascontiguousarray(btype, np.int32))
-    raw = np.ascontiguousarray(raw, np.float32)
-    valid = np.ascontiguousarray(valid, np.int32)
-    cap = 64 + (len(idx) * 3 + 2) * (36 + raw.shape[1] * 8) if len(idx) else 64
-    buf = _outbuf("jobs", cap)
-    blen, nj = ctypes.c_size_t(), ctypes.c_int()
-    rc = load().awmh_stage_jobs(_key(key), _ptr(idx), _ptr(q), _ptr(bt), ctypes.c_size_t(len(idx)), _ptr(raw), _ptr(valid), ctypes.c_int(sample_rate),
-                                buf, ctypes.c_size_t(cap), ctypes.byref(blen), ctypes.byref(nj))
-    if rc:
-        raise RuntimeError("awmh_stage_jobs failed (%d)" % rc)
-    data = ctypes.string_at(buf, blen.value)
-    out, pos = [], 0
-    for _ in range(nj.value):
-        ct, pt, sbt, _pad, time, index_, quality_, n_soft = struct.unpack_from("<BBBBdQdI", data, pos)
-        pos += 32
-        soft = np.frombuffer(data, np.float32, n_soft, pos).copy()
-        pos += 4 * n_soft
-        out.append((ct, pt, sbt, time, index_, quality_, soft))
-    return out
 
 
 def gpu_launches() -> int:

@@ -1,18 +1,24 @@
-"""Plan functions of the multi-GPU run of one long stream (one process per GPU, torch.distributed).
+"""Plan functions of the multi-GPU run of one long stream (one process per GPU).
 
-The sharded `get` itself is C++ (host/awm_balanced.cc: every rank searches an equal slice of the start frames of every chunk its span
-of positions overlaps; three ncclAllGather exchanges of small lists; hostapi.balanced_get).  What lives here is what bench.py and the
+The sharded `get` itself is C++ (host/awm_balanced.cc, reached through hostapi.balanced_get): the reference's 30-minute chunks are
+kept, every rank owns an equal span of stream positions and searches, for each chunk that overlaps its span, the slice of the chunk's
+start frames it owns; three ncclAllGather exchanges of small lists on the context stream.  What lives here is what bench.py and the
 CPU tests need around it: the reference's chunk walk (WavChunkLoader: 30 min, 134.4 s overlap; src/wavchunkloader.cc:54-163), the
-slices of a rank (a mirror of the C++ planner, tests/test_sharding_cpu.py holds the two equal), the range a rank has to embed so that
-its slices read exactly what the unsharded `add` would have written (`add` shards by frame blocks with a recomputed halo: one
-1024-frame for the synthesis window tails, two limiter blocks for the gain ramp), and the blob helpers of the chunk-granular variant.
+slices of a rank and the owner of an index (a mirror of the C++ planner, tests/test_sharding_cpu.py holds the two equal), the input
+range a rank holds, and the range a rank has to embed so that its slices read exactly what the unsharded `add` would have written
+(`add` shards by frame blocks with a recomputed halo: one 1024-frame for the synthesis window tails, two limiter blocks for the gain
+ramp).
 """
 from __future__ import annotations
 
-import os
-import struct
+import math
+
+import numpy as np
 
 FRAME = 1024
+MARK_RATE = 44100              # the watermark rate: a stream at another rate is planned after resampling to it
+T_BLOCK = 2226                 # frames per block (payload 128 bit): sync pattern length in BLOCK mode
+MARGIN = 6                     # start frames of margin on each side of a slice (local mean uses +-20 scores = +-5 frames)
 
 
 def chunk_plan(n_frames: int, max_frames: int, overlap: int, rate: int = 44100):
@@ -34,17 +40,6 @@ def chunk_plan(n_frames: int, max_frames: int, overlap: int, rate: int = 44100):
     return out
 
 
-def assign_chunks(n_chunks: int, world: int):
-    """contiguous, balanced: rank r gets chunks [lo, hi)."""
-    base, extra = divmod(n_chunks, world)
-    out, lo = [], 0
-    for r in range(world):
-        hi = lo + base + (1 if r < extra else 0)
-        out.append((lo, hi))
-        lo = hi
-    return out
-
-
 def embed_range(own_start: int, own_end: int, n_frames: int, limiter_block: int):
     """Extended range [ext_start, ext_end) a rank has to embed so that [own_start, own_end) comes out exactly as in the
     unsharded run.  ext_start is a multiple of 1024 (-> first_frame_number); returns (ext_start, ext_end, first_frame_number).
@@ -63,75 +58,6 @@ def embed_range(own_start: int, own_end: int, n_frames: int, limiter_block: int)
         ext_end = ext_start + -(-(hi - ext_start) // FRAME) * FRAME + FRAME
         ext_end = min(ext_end, n_frames)
     return ext_start, ext_end, ext_start // FRAME
-
-
-def rank_ranges(n_frames: int, rank: int, world: int, max_frames: int, overlap: int, rate: int = 44100):
-    """chunks of this rank and the PCM range [lo, hi) they cover."""
-    plan = chunk_plan(n_frames, max_frames, overlap, rate)
-    lo_c, hi_c = assign_chunks(len(plan), world)[rank]
-    mine = plan[lo_c:hi_c]
-    if not mine:
-        return plan, (lo_c, hi_c), None
-    return plan, (lo_c, hi_c), (mine[0][0], mine[-1][0] + mine[-1][1])
-
-
-# ---- gathering chunk results ---------------------------------------------------------------------------------------
-
-def pack_blobs(blobs) -> bytes:
-    """[(chunk_index, bytes)] -> one byte string."""
-    out = struct.pack("<I", len(blobs))
-    for idx, b in blobs:
-        out += struct.pack("<II", idx, len(b)) + b
-    return out
-
-
-def unpack_blobs(data: bytes):
-    n, = struct.unpack_from("<I", data, 0)
-    pos, out = 4, []
-    for _ in range(n):
-        idx, ln = struct.unpack_from("<II", data, pos)
-        pos += 8
-        out.append((idx, bytes(data[pos:pos + ln])))
-        pos += ln
-    return out
-
-
-def gather_blobs(blobs, device=None):
-    """all ranks -> list over ranks of [(chunk_index, bytes)].  Uses tensor collectives (all_gather of sizes, then of
-    padded byte tensors) so it runs on NCCL (device = cuda) and on gloo (device = None / cpu)."""
-    import torch
-    import torch.distributed as dist
-    payload = pack_blobs(blobs)
-    if not dist.is_initialized() or dist.get_world_size() == 1:
-        return [unpack_blobs(payload)]
-    world = dist.get_world_size()
-    dev = device if device is not None else torch.device("cpu")
-    size = torch.tensor([len(payload)], dtype=torch.int64, device=dev)
-    sizes = [torch.zeros_like(size) for _ in range(world)]
-    dist.all_gather(sizes, size)
-    cap = int(max(int(s.item()) for s in sizes))
-    buf = torch.zeros(cap, dtype=torch.uint8, device=dev)
-    buf[:len(payload)] = torch.frombuffer(bytearray(payload), dtype=torch.uint8).to(dev)
-    bufs = [torch.zeros_like(buf) for _ in range(world)]
-    dist.all_gather(bufs, buf)
-    return [unpack_blobs(bytes(b[:int(s.item())].cpu().numpy().tobytes())) for b, s in zip(bufs, sizes)]
-
-
-# =====================================================================================================================
-# Frame-balanced `get` across ranks: the driver is C++ (audiowmark_b200/host/awm_balanced.cc, reached through
-# hostapi.balanced_get; exchanges = ncclAllGather on the context stream).  Chunk sharding above is exact but coarse
-# (30-minute units); there every rank owns an equal span of stream POSITIONS and searches, for each chunk that overlaps its
-# span, the slice of the chunk's start frames it owns.  The plan functions below restate the C++ ones: bench.py uses them to
-# decide which part of the stream a rank has to hold (and embed), tests/test_sharding_cpu.py checks that both agree.
-# =====================================================================================================================
-
-import math
-
-import numpy as np
-
-MARK_RATE = 44100              # the watermark rate: a stream at another rate is planned after resampling to it
-T_BLOCK = 2226                 # frames per block (payload 128 bit): sync pattern length in BLOCK mode
-MARGIN = 6                     # start frames of margin on each side of a slice (local mean uses +-20 scores = +-5 frames)
 
 
 def owner_span(n_total: int, world: int) -> int:
