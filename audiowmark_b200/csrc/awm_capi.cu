@@ -2877,6 +2877,20 @@ awm_copy_to_host (awm_ctx *ctx, void *dst, const void *src, size_t bytes)
   return 0;
 }
 
+int
+awm_copy (awm_ctx *ctx, void *dst, const void *src, size_t bytes)
+{
+  if (!ctx || (bytes && (!dst || !src)))
+    return fail (ctx, "awm_copy: bad arguments");
+  if (!bytes)
+    return 0;
+  CK (cudaSetDevice (ctx->device));
+  CK (cudaMemcpyAsync (dst, src, bytes, cudaMemcpyDefault, ctx->stream));
+  if (!is_device_ptr (src))
+    CK (cudaStreamSynchronize (ctx->stream));       /* a pinned host source is read asynchronously: the caller may reuse it next */
+  return 0;
+}
+
 /* ---------------------------------------------------------------- batched embed */
 
 namespace {

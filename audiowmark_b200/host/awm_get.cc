@@ -3,6 +3,7 @@
 // Viterbi decoder run on the GPU through the C ABI; pairing / combining logic stays on the host.
 #include "awm_results.hh"
 #include "awm_get_internal.hh"
+#include "awm_balanced.hh"
 #include "awm_speed.hh"
 #include "awm_engine.hh"
 #include "awm_tables.hh"
@@ -535,6 +536,256 @@ chunk_geometry (int sample_rate, size_t& max_frames, size_t& overlap_frames)
   overlap_frames = lrint (2 * block_seconds * 1.3 * sample_rate);
 }
 
+/* ---------------------------------------------------------------- GetStream */
+
+namespace {
+
+constexpr size_t kInputWindow = size_t (1) << 20;      // input frames the window takes between two resampler launches
+
+/* buf[0, n) = buf[from, from + n) (frames of `channels` floats, device memory) in context stream order, in copies that do not
+ * overlap: each reads frames no earlier copy has written */
+bool
+move_to_front (awm_ctx *ctx, float *buf, size_t from, size_t n, int channels)
+{
+  for (size_t done = 0; done < n && from; )
+    {
+      const size_t k = min (n - done, from);
+      if (awm_copy (ctx, buf + done * channels, buf + (from + done) * channels, k * channels * sizeof (float)))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return false;
+        }
+      done += k;
+    }
+  return true;
+}
+
+}
+
+GetStream::GetStream (const vector<Key>& key_list, int n_channels, int sample_rate, bool print_speed_results, size_t max_input_frames, bool dry_run) :
+  m_keys (key_list), m_channels (n_channels), m_rate (sample_rate), m_print_speed (print_speed_results), m_dry (dry_run), m_max_input (max_input_frames)
+{
+  if (n_channels <= 0)
+    {
+      error ("audiowmark: get: %d channels\n", n_channels);
+      return;
+    }
+  if (!balanced::rate_supported (sample_rate))
+    {
+      error ("audiowmark: get: sample rate %d Hz is not supported (%d Hz / 64 .. %d Hz * 64, exclusive)\n", sample_rate, Params::mark_sample_rate,
+             Params::mark_sample_rate);
+      return;
+    }
+  m_ratio = double (Params::mark_sample_rate) / sample_rate;
+  chunk_geometry (Params::mark_sample_rate, m_max_frames, m_overlap);
+  if (m_overlap >= m_max_frames)
+    {
+      error ("audiowmark: get: chunks of %zu frames cannot overlap by %zu frames\n", m_max_frames, m_overlap);
+      return;
+    }
+  m_ok = true;
+}
+
+GetStream::~GetStream()
+{
+  if (m_chunk || m_in)
+    {
+      awm_device_free (Engine::ctx(), m_chunk);
+      awm_device_free (Engine::ctx(), m_in);
+    }
+}
+
+/* the chunk buffer (watermark rate, at most one chunk, or the whole announced stream if shorter) and at other rates the input window,
+ * allocated once with the first fed frame: the stream's length does not change them */
+bool
+GetStream::ensure_buffers()
+{
+  if (m_chunk_cap)
+    return true;
+  m_chunk_cap = m_max_input == ~size_t (0) ? m_max_frames : min (m_max_frames, balanced::mark_frames (m_max_input, m_rate));
+  if (m_rate != Params::mark_sample_rate)
+    {
+      /* the taps of the next output start at most 2h - 1 frames before the input's end (awm_resample_stream_available), plus one frame
+       * of margin as in balanced::input_range */
+      const size_t h = size_t (ceil (16 / std::min (1.0, m_ratio)));
+      m_in_cap = min (kInputWindow, m_max_input) + 2 * h + 2;
+    }
+  m_peak_bytes = (m_chunk_cap + m_in_cap) * m_channels * sizeof (float);
+  if (m_dry)
+    return true;
+  awm_ctx *ctx = Engine::ctx();
+  void *chunk = nullptr, *in = nullptr;
+  if (!ctx || awm_device_alloc (ctx, m_chunk_cap * m_channels * sizeof (float), &chunk)
+      || (m_in_cap && awm_device_alloc (ctx, m_in_cap * m_channels * sizeof (float), &in)))
+    {
+      if (ctx)
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          awm_device_free (ctx, chunk);
+        }
+      return false;
+    }
+  m_chunk = static_cast<float *> (chunk);
+  m_in = static_cast<float *> (in);
+  return true;
+}
+
+/* decode the chunk buffer's m_fill frames as chunk number m_chunks.size() */
+bool
+GetStream::decode()
+{
+  const int chunk = int (m_chunks.size());
+  m_chunks.push_back ({ m_start, m_fill, m_time_offset });
+  string debug_sync;
+  if (!m_dry)
+    {
+      PcmRef pcm;
+      pcm.f32 = m_chunk;
+      if (decode_chunk (m_pending, chunk, debug_sync, m_keys, pcm, m_fill, m_channels, Params::mark_sample_rate, chunk == 0, m_print_speed, -1))
+        return false;
+    }
+  m_debug_syncs.push_back (debug_sync);
+  return true;
+}
+
+/* a full chunk is decoded; the next one starts with its last m_overlap frames */
+bool
+GetStream::chunk_full()
+{
+  if (!decode() || (!m_dry && !move_to_front (Engine::ctx(), m_chunk, m_max_frames - m_overlap, m_overlap, m_channels)))
+    return false;
+  m_fill = m_overlap;
+  m_start += m_max_frames - m_overlap;
+  m_time_offset += double (m_max_frames - m_overlap) / Params::mark_sample_rate;
+  return true;
+}
+
+/* resample the watermark-rate frames [m_produced, until) into the chunk buffer from the input window; the caller guarantees that their
+ * taps lie in [m_in_first, m_fed), so they are what awm_resample over the whole stream computes, whatever its final length */
+bool
+GetStream::produce (size_t until)
+{
+  awm_ctx *ctx = m_dry ? nullptr : Engine::ctx();
+  while (m_produced < until)
+    {
+      const size_t n = min (until - m_produced, m_max_frames - m_fill);
+      if (ctx && awm_resample_range (ctx, m_in, m_in_first, m_fed - m_in_first, m_fed, m_channels, m_ratio, 16, m_chunk + m_fill * m_channels, m_produced, n))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return false;
+        }
+      m_produced += n;
+      m_fill += n;
+      if (m_fill == m_max_frames && !chunk_full())
+        return false;
+    }
+  return true;
+}
+
+int
+GetStream::feed (const float *pcm, size_t n_frames)
+{
+  if (!m_ok || m_failed || m_finished || (!pcm && n_frames && !m_dry) || n_frames > m_max_input - min (m_fed, m_max_input))
+    {
+      error ("audiowmark: get: cannot feed %zu frames to this stream (%s)\n", n_frames, !m_ok ? "refused" : m_failed ? "failed before"
+             : m_finished ? "finished" : !pcm ? "no samples" : "more frames than announced");
+      m_failed = true;
+      return 1;
+    }
+  if (n_frames && !ensure_buffers())
+    {
+      m_failed = true;
+      return 1;
+    }
+  awm_ctx *ctx = m_dry ? nullptr : Engine::ctx();
+  const size_t C = m_channels;
+  while (n_frames)
+    {
+      size_t n;
+      if (m_rate == Params::mark_sample_rate)
+        {
+          n = min (n_frames, m_max_frames - m_fill);
+          if (ctx && awm_copy (ctx, m_chunk + m_fill * C, pcm, n * C * sizeof (float)))
+            break;
+          m_fed += n;
+          m_produced += n;
+          m_fill += n;
+          if (m_fill == m_max_frames && !chunk_full())
+            {
+              m_failed = true;
+              return 1;
+            }
+        }
+      else
+        {
+          if (m_fed - m_in_first == m_in_cap)
+            {
+              /* the window is full: make every output it can, then keep only the input the taps of later outputs read */
+              uint64_t t0, t1;
+              if (!produce (resample_stream_available (m_fed, m_ratio)))
+                {
+                  m_failed = true;
+                  return 1;
+                }
+              awm_resample_taps (m_fed, m_ratio, 16, m_produced, 1, &t0, &t1);
+              const size_t keep = std::max (m_in_first, t0 ? size_t (t0) - 1 : 0);
+              if (ctx && !move_to_front (ctx, m_in, keep - m_in_first, m_fed - keep, m_channels))
+                {
+                  m_failed = true;
+                  return 1;
+                }
+              m_in_first = keep;
+            }
+          n = min (n_frames, m_in_cap - (m_fed - m_in_first));
+          if (ctx && awm_copy (ctx, m_in + (m_fed - m_in_first) * C, pcm, n * C * sizeof (float)))
+            break;
+          m_fed += n;
+        }
+      if (pcm)
+        pcm += n * C;
+      n_frames -= n;
+    }
+  if (n_frames)
+    {
+      error ("audiowmark: %s\n", awm_last_error (ctx));
+      m_failed = true;
+      return 1;
+    }
+  return 0;
+}
+
+int
+GetStream::finish (ResultSet& result_set, size_t *mark_rate_frames)
+{
+  if (!m_ok || m_failed || m_finished)
+    {
+      error ("audiowmark: get: cannot finish this stream (%s)\n", !m_ok ? "refused" : m_failed ? "failed before" : "finished");
+      return 1;
+    }
+  m_finished = true;
+  /* at EOF the resampler delivers its trailing outputs: those of the whole stream, now that its length is known */
+  if (m_rate != Params::mark_sample_rate && m_fed && !produce (balanced::mark_frames (m_fed, m_rate)))
+    return 1;
+  if ((!m_chunks.empty() || m_fill) && !decode())
+    return 1;
+  if (mark_rate_frames)
+    *mark_rate_frames = m_produced;
+  if (m_dry || m_chunks.empty())
+    return 0;
+  /* one Viterbi launch, then the reference's per-chunk merge in chunk order */
+  vector<ResultSet> chunk_results (m_chunks.size());
+  if (!run_viterbi_jobs (m_pending, chunk_results))
+    return 1;
+  for (size_t c = 0; c < chunk_results.size(); c++)
+    {
+      chunk_results[c].set_debug_sync (m_debug_syncs[c]);
+      chunk_results[c].apply_time_offset (m_chunks[c].time_offset);
+      result_set.merge (chunk_results[c]);
+    }
+  result_set.sort (m_keys);
+  return 0;
+}
+
 int
 get_watermark_buffer (const vector<Key>& key_list, const float *samples, size_t n_frames, int n_channels, int sample_rate, ResultSet& result_set,
                       bool print_speed_results, size_t *mark_rate_frames)
@@ -553,35 +804,24 @@ int
 get_watermark_pcm (const vector<Key>& key_list, const float *samples, const int16_t *samples16, size_t n_frames, int n_channels, int sample_rate,
                    ResultSet& result_set, bool print_speed_results, size_t *mark_rate_frames)
 {
-  vector<float> resampled, converted;
-  if (samples16 && sample_rate != Params::mark_sample_rate)
-    {
-      /* rare combination: convert on the host, then take the float path through the resampler */
-      converted.resize (n_frames * n_channels);
-      const float norm = 1.0 / 0x80000000LL;
-      for (size_t i = 0; i < converted.size(); i++)
-        converted[i] = (int (samples16[i]) << 16) * norm;
-      samples = converted.data();
-      samples16 = nullptr;
-    }
   if (sample_rate != Params::mark_sample_rate)
     {
-      /* WavChunkLoader resamples the input to the watermark rate while it reads (src/wavchunkloader.cc:66-73, 196-221) */
-      const double ratio = double (Params::mark_sample_rate) / sample_rate;
-      awm_ctx *rctx = Engine::ctx();
-      if (!rctx)
-        return 1;
-      const size_t n_out = resample_stream_frames (n_frames, ratio);
-      resampled.assign (n_out * n_channels, 0.f);
-      if (awm_resample (rctx, samples, n_frames, n_channels, ratio, 16, resampled.data(), n_out))
+      /* WavChunkLoader resamples the input to the watermark rate while it reads (src/wavchunkloader.cc:66-73, 196-221): the whole
+       * buffer is one piece of a stream, resampled chunk by chunk on the device */
+      vector<float> converted;
+      if (samples16)
         {
-          error ("audiowmark: %s\n", awm_last_error (rctx));
-          return 1;
+          /* rare combination: convert on the host, then take the float path through the resampler */
+          converted.resize (n_frames * n_channels);
+          const float norm = 1.0 / 0x80000000LL;
+          for (size_t i = 0; i < converted.size(); i++)
+            converted[i] = (int (samples16[i]) << 16) * norm;
+          samples = converted.data();
         }
-      samples = resampled.data();
-      samples16 = nullptr;
-      n_frames = n_out;
-      sample_rate = Params::mark_sample_rate;
+      GetStream stream (key_list, n_channels, sample_rate, print_speed_results, n_frames);
+      if (!stream.ok() || stream.feed (samples, n_frames))
+        return 1;
+      return stream.finish (result_set, mark_rate_frames);
     }
   if (mark_rate_frames)
     *mark_rate_frames = n_frames;
@@ -701,24 +941,38 @@ get_watermark (const vector<Key>& key_list, const string& infile, const string& 
       if (orig_bitvec.empty())
         return 1;
     }
-  /* the reference streams chunk by chunk to bound host memory; device memory holds hours of audio, so the file is
-   * read once and the same chunk geometry is applied to the buffer */
-  WavData wav;
-  Error err = wav.load (infile);
+  Error err;
+  std::unique_ptr<AudioInputStream> in = AudioInputStream::create (infile, err);
   if (err)
     {
       error ("audiowmark: error loading %s: %s\n", infile.c_str(), err.message());
       return 1;
     }
-  if (Params::test_truncate)
+  /* --test-truncate: the first sample_rate * seconds frames */
+  const size_t limit = Params::test_truncate ? size_t (in->sample_rate()) * Params::test_truncate : ~size_t (0);
+  GetStream stream (key_list, in->n_channels(), in->sample_rate(), !orig_bitvec.empty(),
+                    in->n_frames() == AudioInputStream::N_FRAMES_UNKNOWN ? limit : min (in->n_frames(), limit));
+  if (!stream.ok())
+    return 1;
+  vector<float> piece;
+  for (size_t frames = 0; frames < limit; )
     {
-      const size_t want = size_t (wav.sample_rate()) * wav.n_channels() * Params::test_truncate;
-      if (want < wav.n_values())
-        wav.mutable_samples().resize (want);
+      err = in->read_frames (piece, min<size_t> (limit - frames, 1 << 18));
+      if (err)
+        {
+          error ("audiowmark: error loading %s: %s\n", infile.c_str(), err.message());
+          return 1;
+        }
+      if (piece.empty())
+        break;
+      const size_t n = piece.size() / in->n_channels();
+      if (stream.feed (piece.data(), n))
+        return 1;
+      frames += n;
     }
   ResultSet result_set;
   size_t mark_rate_frames = 0;
-  if (get_watermark_buffer (key_list, wav.samples().data(), wav.n_frames(), wav.n_channels(), wav.sample_rate(), result_set, !orig_bitvec.empty(), &mark_rate_frames))
+  if (stream.finish (result_set, &mark_rate_frames))
     return 1;
   const size_t time_length = lrint (mark_rate_frames / double (Params::mark_sample_rate));
   return report (result_set, time_length, orig_bitvec);

@@ -432,6 +432,81 @@ awmh_get (const unsigned char *keys16, const char *const *names, int n_keys, con
   return result_json (result_set, mark_rate_frames, json_out, json_cap, n_patterns);
 }
 
+static std::vector<Key> make_key_list (const unsigned char *keys16, const char *const *names, int n_keys);
+
+/* ---- streaming `get` (GetStream): a stream fed piece by piece in bounded memory -------------------------------------------------
+ * awmh_gs_create returns NULL, with a message and without GPU work, for a sample rate outside the resampler's range or channels <= 0.
+ * awmh_gs_feed takes interleaved float frames in host or device memory; awmh_gs_finish writes the --json document as awmh_get does.
+ * After a failed feed, or after finish, the stream only accepts awmh_gs_destroy. */
+void *
+awmh_gs_create (const unsigned char *keys16, const char *const *names, int n_keys, int n_channels, int sample_rate, int print_speed_results)
+{
+  GetStream *s = new GetStream (make_key_list (keys16, names, n_keys), n_channels, sample_rate, print_speed_results != 0);
+  if (!s->ok())
+    {
+      delete s;
+      return nullptr;
+    }
+  return s;
+}
+
+int
+awmh_gs_feed (void *h, const float *pcm, size_t n_frames)
+{
+  return static_cast<GetStream *> (h)->feed (pcm, n_frames);
+}
+
+int
+awmh_gs_finish (void *h, char *json_out, size_t json_cap, int *n_patterns)
+{
+  ResultSet result_set;
+  size_t mark_rate_frames = 0;
+  const int rc = static_cast<GetStream *> (h)->finish (result_set, &mark_rate_frames);
+  if (rc)
+    return rc;
+  return result_json (result_set, mark_rate_frames, json_out, json_cap, n_patterns);
+}
+
+void
+awmh_gs_destroy (void *h)
+{
+  delete static_cast<GetStream *> (h);
+}
+
+/* device bytes the stream holds at most (chunk buffer + input window) */
+uint64_t
+awmh_gs_peak_bytes (void *h)
+{
+  return static_cast<GetStream *> (h)->peak_device_bytes();
+}
+
+/* test aid (CPU): the chunks GetStream decodes for a stream of n_total frames at sample_rate fed in pieces of piece_frames, without a
+ * device (chunks [max][3]: first frame, frames, time offset, in watermark-rate frames); *mark_frames: the stream's watermark-rate length.
+ * Returns 1 for a refused rate */
+int
+awmh_gs_plan (uint64_t n_total, uint64_t piece_frames, int sample_rate, double *chunks, int max_chunks, int *n_chunks, uint64_t *mark_frames)
+{
+  GetStream s ({}, 1, sample_rate, false, ~size_t (0), true);
+  if (!s.ok() || !piece_frames)
+    return 1;
+  for (uint64_t fed = 0; fed < n_total; fed += piece_frames)
+    if (s.feed (nullptr, std::min (piece_frames, n_total - fed)))
+      return 1;
+  ResultSet rs;
+  size_t m = 0;
+  if (s.finish (rs, &m))
+    return 1;
+  *mark_frames = m;
+  *n_chunks = int (s.chunks().size());
+  for (int c = 0; c < *n_chunks && c < max_chunks; c++)
+    {
+      chunks[3 * c] = double (s.chunks()[c].first);
+      chunks[3 * c + 1] = double (s.chunks()[c].n_frames);
+      chunks[3 * c + 2] = s.chunks()[c].time_offset;
+    }
+  return 0;
+}
+
 static int
 result_json (ResultSet& result_set, size_t mark_rate_frames, char *json_out, size_t json_cap, int *n_patterns)
 {

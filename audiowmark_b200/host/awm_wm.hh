@@ -70,6 +70,57 @@ int add_watermark_buffer_s16 (const Key& key, const int16_t *in, int16_t *out, s
 /* the reference's chunks (WavChunkLoader geometry), which get_watermark_buffer and the sharded `get` both walk */
 void chunk_geometry (int sample_rate, size_t& max_frames, size_t& overlap_frames);
 
+namespace get_detail { struct VitJob; }
+
+/* One `get` over a stream that arrives piece by piece (a pipe, a long file), in bounded memory: the chunk loop of WavChunkLoader
+ * (src/wavchunkloader.cc:112-239).  Fed frames (interleaved float, host or device) go into one device chunk buffer of max_frames
+ * frames at the watermark rate; at other rates they pass a small device input window and are resampled into it (awm_resample_range)
+ * bit for bit as awm_resample of the whole stream would.  A chunk is decoded when it is full, the next one starts with its last
+ * `overlap` frames, and the last one is only known at finish (a stream that exactly fills a chunk gives one more, overlap-only
+ * chunk; an empty stream none).  finish runs the Viterbi decoder once over all chunks and merges their results in chunk order, as
+ * get_watermark_buffer does.  max_input_frames (optional): the stream has at most that many frames, so a short stream gets a chunk
+ * buffer of its own size.  dry_run: no device work at all, only the chunk decisions (chunks()), for tests without a GPU. */
+class GetStream
+{
+public:
+  struct Chunk { size_t first, n_frames; double time_offset; };     // watermark-rate frames
+
+  GetStream (const std::vector<Key>& key_list, int n_channels, int sample_rate, bool print_speed_results,
+             size_t max_input_frames = ~size_t (0), bool dry_run = false);
+  ~GetStream();
+  GetStream (const GetStream&) = delete;
+  GetStream& operator= (const GetStream&) = delete;
+
+  bool ok() const { return m_ok; }                 // false: refused at construction, with a message
+  int  feed (const float *pcm, size_t n_frames);    // 0, or 1 with a message (the stream is then unusable)
+  int  finish (ResultSet& result_set, size_t *mark_rate_frames);
+  const std::vector<Chunk>& chunks() const { return m_chunks; }
+  size_t peak_device_bytes() const { return m_peak_bytes; }
+
+private:
+  bool ensure_buffers();
+  bool chunk_full();
+  bool produce (size_t until);
+  bool decode();
+
+  std::vector<Key> m_keys;
+  int    m_channels, m_rate;
+  bool   m_print_speed, m_dry, m_ok = false, m_failed = false, m_finished = false;
+  double m_ratio = 1;                    // watermark rate / input rate
+  size_t m_max_frames = 0, m_overlap = 0, m_max_input = 0;
+  size_t m_fill = 0, m_fed = 0, m_produced = 0;
+  size_t m_start = 0;                    // watermark-rate frame of the chunk buffer's first frame
+  double m_time_offset = 0;
+  float *m_chunk = nullptr;              // [m_chunk_cap][channels], device
+  size_t m_chunk_cap = 0;
+  float *m_in = nullptr;                 // input window [m_in_cap][channels], device: stream frames [m_in_first, m_fed)
+  size_t m_in_cap = 0, m_in_first = 0;
+  size_t m_peak_bytes = 0;
+  std::vector<Chunk> m_chunks;
+  std::vector<std::string> m_debug_syncs;
+  std::vector<get_detail::VitJob> m_pending;
+};
+
 int frame_count (const WavData& wav_data);
 
 class SyncFinder

@@ -18,7 +18,8 @@ CLI_PATH = os.path.join(_HERE, "bin", "audiowmark")
 EXPORTS = ["awmh_set_params", "awmh_frames_per_block", "awmh_n_coded_bits", "awmh_random_u64", "awmh_gen_noise", "awmh_sync_table",
            "awmh_mix_table", "awmh_frame_mod", "awmh_conv_encode", "awmh_add", "awmh_get", "awmh_merge_chunks", "awmh_chunk_geometry", "awmh_ctx", "awmh_key_slot", "awmh_stage_select", "awmh_gpu_launches", "awmh_gpu_stream", "awmh_synchronize", "awmh_profile_enable", "awmh_profile_report", "awmh_shutdown", "awmh_set_speed_params", "awmh_detect_speed", "awmh_resample", "awmh_resample_stream_frames", "awmh_resample_stream_available", "awmh_resampled_add_plan", "awmh_set_short_payload", "awmh_add_s16", "awmh_get_s16", "awmh_short_encode", "awmh_short_decode", "awmh_sync_trace", "awmh_sync_trace_fetch", "awmh_dist_unique_id", "awmh_dist_init", "awmh_balanced_get", "awmh_bg_create", "awmh_bg_destroy", "awmh_bg_stage", "awmh_bg_plan", "awmh_bg_owner", "awmh_bg_input_range", "awmh_add_windowed",
            "awmh_embed_roles", "awmh_coded_bits", "awmh_add_batch", "awmh_role_layout", "awmh_embed_roles_device",
-           "awmh_window_range", "awmh_add_window"]
+           "awmh_window_range", "awmh_add_window", "awmh_gs_create", "awmh_gs_feed", "awmh_gs_finish", "awmh_gs_destroy", "awmh_gs_peak_bytes",
+           "awmh_gs_plan"]
 
 _lib = None
 
@@ -33,6 +34,8 @@ def load():
         lib.awmh_gpu_launches.restype = ctypes.c_uint64
         lib.awmh_gpu_stream.restype = ctypes.c_void_p
         lib.awmh_ctx.restype = ctypes.c_void_p
+        lib.awmh_gs_create.restype = ctypes.c_void_p
+        lib.awmh_gs_peak_bytes.restype = ctypes.c_uint64
         _lib = lib
     return _lib
 
@@ -401,6 +404,90 @@ def get(pcm, keys=None, names=None, n_frames=None, channels=None, sample_rate=44
         raise RuntimeError("awmh_get failed (rc=%d); see stderr" % rc)
     text = buf.value.decode()
     return json.loads(text) if parse else text
+
+
+class GetStream:
+    """`get` over a stream that arrives piece by piece (a pipe, a long recording), in bounded memory: the pieces go into one device
+    chunk buffer (at other rates through a small device input window and the resampler), each chunk is decoded once it is full, and
+    finish() returns the --json document (parse=False: its text) of get() on the whole stream, byte for byte.  feed(pcm) takes a
+    numpy array [n, channels] (float32) or a float32 device pointer with n_frames.  ValueError for a sample rate outside the resampler's
+    range, a channel count that does not match and a feed or finish after finish."""
+
+    def __init__(self, keys=None, names=None, channels=2, sample_rate=44100):
+        keys = keys or [bytes(16)]
+        names = names or [""] * len(keys)
+        self.channels, self.sample_rate, self._finished = int(channels), int(sample_rate), False
+        kb = b"".join(_key(k) for k in keys)
+        name_arr = (ctypes.c_char_p * len(keys))(*[n.encode() for n in names])
+        self.h = load().awmh_gs_create(kb, name_arr, ctypes.c_int(len(keys)), ctypes.c_int(self.channels), ctypes.c_int(self.sample_rate), ctypes.c_int(0))
+        if not self.h:
+            raise ValueError("GetStream: %d channels at %d Hz are not supported; see stderr" % (self.channels, self.sample_rate))
+
+    def _check(self, what):
+        if self.h is None:
+            raise ValueError("GetStream.%s: the stream is closed" % what)
+        if self._finished:
+            raise ValueError("GetStream.%s: the stream is finished" % what)
+
+    def feed(self, pcm, n_frames=None):
+        self._check("feed")
+        if isinstance(pcm, np.ndarray):
+            if pcm.ndim != 2 or pcm.shape[1] != self.channels:
+                raise ValueError("GetStream.feed: expected [n, %d] frames, got shape %s" % (self.channels, pcm.shape))
+            pcm = np.ascontiguousarray(pcm, np.float32)
+            n_frames = pcm.shape[0]
+        elif n_frames is None:
+            raise ValueError("GetStream.feed: a device pointer needs n_frames")
+        rc = load().awmh_gs_feed(ctypes.c_void_p(self.h), _ptr(pcm), ctypes.c_size_t(int(n_frames)))
+        if rc:
+            raise RuntimeError("awmh_gs_feed failed (rc=%d); see stderr" % rc)
+
+    def finish(self, parse=True):
+        self._check("finish")
+        self._finished = True
+        cap = 1 << 22
+        buf = _outbuf("get", cap)
+        n_pat = ctypes.c_int()
+        rc = load().awmh_gs_finish(ctypes.c_void_p(self.h), buf, ctypes.c_size_t(cap), ctypes.byref(n_pat))
+        if rc:
+            raise RuntimeError("awmh_gs_finish failed (rc=%d); see stderr" % rc)
+        text = buf.value.decode()
+        return json.loads(text) if parse else text
+
+    def peak_bytes(self) -> int:
+        """device bytes the stream holds at most: its chunk buffer plus, at other rates, its input window"""
+        if self.h is None:
+            raise ValueError("GetStream.peak_bytes: the stream is closed")
+        return int(load().awmh_gs_peak_bytes(ctypes.c_void_p(self.h)))
+
+    def close(self):
+        if self.h:
+            load().awmh_gs_destroy(ctypes.c_void_p(self.h))
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        if getattr(self, "h", None) and _lib is not None:
+            self.close()
+
+
+def get_stream_plan(n_total: int, piece_frames: int, sample_rate=44100):
+    """test aid (CPU): the chunks GetStream decodes for a stream of n_total frames fed in pieces of piece_frames, without a device ->
+    ([(first, n_frames, time_offset)], watermark-rate length), frames at the watermark rate"""
+    cap = 4096
+    chunks = np.zeros((cap, 3), np.float64)
+    n, m = ctypes.c_int(), ctypes.c_uint64()
+    if load().awmh_gs_plan(ctypes.c_uint64(n_total), ctypes.c_uint64(piece_frames), ctypes.c_int(sample_rate), _ptr(chunks), ctypes.c_int(cap),
+                           ctypes.byref(n), ctypes.byref(m)):
+        raise ValueError("get_stream_plan: sample rate %d Hz or piece size %d refused" % (sample_rate, piece_frames))
+    if n.value > cap:
+        raise ValueError("get_stream_plan: more than %d chunks" % cap)
+    return [(int(a), int(b), float(t)) for a, b, t in chunks[:n.value]], m.value
 
 
 def sync_trace(on=True):

@@ -426,6 +426,10 @@ int awm_pcm_pop (awm_ctx *ctx);
 /* stream ordered copy device (or host) -> host for callers that keep their PCM in device memory but need a few values on
  * the host (clip selection of detect_speed hashes a sparse subset of the samples, src/wmspeed.cc:533-552) */
 int awm_copy_to_host (awm_ctx *ctx, void *dst, const void *src, size_t bytes);
+/* copy of `bytes` between any two buffers (host or device, not overlapping) in context stream order: it runs after the work queued
+ * before it and the work queued after it sees the result.  Returns at once for a device source; a host source may be reused when it
+ * returns (streaming `get`: pieces of a pipe go into the device chunk buffer as they arrive) */
+int awm_copy (awm_ctx *ctx, void *dst, const void *src, size_t bytes);
 /* dst_host[k] = src[indices[k]] for a device resident src (the sample subset detect_speed hashes) */
 int awm_gather (awm_ctx *ctx, const float *src, const uint64_t *indices, size_t n, float *dst_host);
 /* 1 if p points to CUDA device / managed memory (such pointers are used in place by the PCM entry points), else 0 */
