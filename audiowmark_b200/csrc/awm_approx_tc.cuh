@@ -11,12 +11,20 @@
 //     every product with a 0/1 mask element is exact, accumulation is fp32
 //   * B operand = the 0/1 masks of 48 entries (96 columns: U and D of an entry side by side), prepared once per key on the host in
 //     operand layout and fetched chunk by chunk with the bulk-copy engine (TMA, cp.async.bulk -> mbarrier complete_tx)
-//   * D = 64 x 32 fp32 blocks in the registers of the MMA warpgroup, which writes them to `mags` itself
+//   * D = one 64 x 96 fp32 accumulator per 64-row half of the tile and chunk (48 registers per thread) in the registers of the
+//     MMA warpgroup, which writes it to `mags` itself; the stores of the second half run under the bulk copy of the next mask chunk
 // Warp roles (one CTA per SM, CTAs walk the (frame tile, shift) list with stride gridDim.x):
 //   warps 0 .. 11      FFT: frame (PCM prefetched by TMA into the warp's transpose buffer) -> packed 1024-point FFT -> dB ->
 //                      fp16 hi/lo into A[buf]                                                     (a_empty -> a_full)
-//   warps 12 .. 15     one warpgroup: B chunk loads (thread 0), wgmma per 64 x 32 block, stores   (a_full, b_full -> a_empty)
+//   warps 12 .. 15     one warpgroup: B chunk loads (thread 0), 2 x 12 m64n96k16 wgmma per chunk, stores
+//                                                                                                 (a_full, b_full -> a_empty)
 // All hand-offs are mbarriers; the FFT of tile i + 1 overlaps the MMAs and the stores of tile i.
+// Shared memory (225.25 KB of the 227 KB an SM grants one CTA):
+//   twiddles 8 KB | window 4 KB | 12 transpose / PCM landing buffers of 8448 B (99 KB) | 2 A buffers of 48 KB (hi 24 KB + lo 24 KB)
+//   | 1 B buffer of 18 KB (one mask chunk) | mbarriers (256 B)
+// A second B buffer does not fit, so the next chunk's masks are fetched into the one buffer once the chunk's last wgmma retired.
+// Operand bytes per wgmma: A 2 KB (64 rows x 16 K), B 3 KB (96 columns x 16 K); per 128-frame tile 11 chunks x 24 wgmma read
+// 22 x 12 A blocks (0.53 MB) and 11 x 24 B blocks (0.79 MB) -- tools/stft_smem_model.py counts them against the FFT warps' bytes.
 #pragma once
 #include "awm_kernels.cuh"
 #include "awm_tc.cuh"
@@ -29,7 +37,6 @@ constexpr int kTcK = 96;                     // 81 bands padded to a multiple of
 constexpr uint32_t kTcASplit = kTcTile * kTcK * 2;        // bytes of one fp16 term of the A tile (24 KB)
 constexpr uint32_t kTcABytes = 2 * kTcASplit;             // hi + lo
 constexpr int kTcEpiWarps = 4;             // the MMA warpgroup
-constexpr int kTcNB = 32;                  // columns (16 entries) per wgmma block
 constexpr int kTcFftWarps = 12;
 constexpr int kTcABufs = 2;                // the FFT of tile i + 1 fills one A buffer while the MMAs read tile i from the other
 // sync entries per B chunk -> N = 2 kTcChunkEnt columns (U and D column of every entry), chunk of N x 96 fp16 (18 KB): small
@@ -39,7 +46,7 @@ constexpr int kTcN = 2 * kTcChunkEnt;
 constexpr uint32_t kTcBBytes = uint32_t (kTcN) * kTcK * 2;
 constexpr size_t kTcSmemBytes = fft_smem_bytes (kTcFftWarps) + size_t (kTcABufs) * kTcABytes + kTcBBytes + 256;
 static_assert (kTcFftWarps % 4 == 0, "the MMA warpgroup has to start at a warp index divisible by four");
-static_assert (kTcN % kTcNB == 0, "a chunk is a whole number of wgmma blocks");
+static_assert (kTcN == 96, "one m64n96k16 wgmma covers the columns of a chunk");
 
 // host side: the 0/1 masks of all entries in operand layout, chunk after chunk ([ceil (n_ent / kTcChunkEnt)][kTcBBytes])
 inline void
@@ -214,15 +221,53 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
   else
     {
       // ===================================================================================== MMA warpgroup
-      // Per chunk: 2 (64-row halves) x kTcN / 32 (column blocks) x [2 (hi, lo) x 6 (K steps)] wgmma, each block written to `mags`
-      // as soon as it is complete.  The mask chunk has one buffer: thread 0 loads the next chunk as soon as the whole warpgroup is
-      // past the last MMA that reads the current one, and the load lands while the last blocks are stored.
+      // Per chunk and 64-row half: ONE 64 x 96 accumulator (all 48 entries of the chunk), built by 2 (hi, lo) x 6 (K steps)
+      // m64n96k16 wgmma in that order, so an element sees the same products in the same order as in any narrower split of the
+      // columns.  Half 0 is computed and stored, then half 1; once half 1 has retired nothing reads the mask chunk any more,
+      // thread 0 starts the bulk copy of the next chunk into the one B buffer, and half 1 is stored while it lands.  (Keeping both
+      // halves in flight -- 96 accumulators, half 0 stored under the MMAs of half 1 -- measured slower: the extra registers cost
+      // the FFT warps spills in their frame loop.)
       const int wt = threadIdx.x - kTcFftWarps * 32, wi = wt >> 5;                  // thread / warp within the warpgroup
       const uint32_t b_addr = smem_u32 (bbuf);
       auto load_b = [&] (int c)
         {
           mbar_arrive_expect_tx (b_full, kTcBBytes);
           bulk_load (bbuf, masks + size_t (c) * kTcBBytes, kTcBBytes, b_full);
+        };
+      // the descriptors of all 24 wgmma of a chunk are one base descriptor per operand plus a constant (the start address sits in
+      // the low bits, in units of 16 bytes, and never carries out of its field).  The A base is re-derived behind an empty asm in
+      // every chunk, so the compiler does not keep 24 loop-invariant descriptors live next to the accumulators.
+      auto mma_half = [&] (float (&d)[kTcN / 2], uint64_t da, uint64_t db, int mh)
+        {
+#pragma unroll
+          for (int sp = 0; sp < 2; sp++)
+#pragma unroll
+            for (int j = 0; j < kTcK / 16; j++)
+              wgmma_m64n96k16_f16 (d, da + ((sp * kTcASplit + j * 2 * (kTcTile * 16) + mh * (64 / 8) * 128) >> 4),
+                                   db + ((j * 2 * (kTcN * 16)) >> 4), (sp | j) != 0);
+          wgmma_commit();
+        };
+      auto store_half = [&] (float (&d)[kTcN / 2], int shift_idx, int f0, int c, int mh)
+        {
+#pragma unroll
+          for (int i = 0; i < kTcN / 2; i++)
+            wgmma_fence_operand (d[i]);
+          asm volatile ("" : "+r"(c));              // the addresses are formed here, after the wait, not held across the MMAs
+          const int e_base = c * kTcChunkEnt + (lane & 3);
+          const int f = f0 + mh * 64 + wi * 16 + (lane >> 2);                   // f + 8 < ld always (ld multiple of 128)
+#pragma unroll
+          for (int q = 0; q < kTcN / 8; q++)
+            {
+              const int e = e_base + 4 * q;
+              if (e < n_ent)
+                {
+                  // streaming stores (evict first): the 1.27 GB of entry sums per chunk pass through L2 without pushing out the
+                  // PCM frames and mask chunks that the bulk copies read again
+                  float2 *row = mags + ((size_t) shift_idx * n_ent + e) * ld + f;
+                  __stcs (row, make_float2 (d[4 * q], d[4 * q + 1]));
+                  __stcs (row + 8, make_float2 (d[4 * q + 2], d[4 * q + 3]));
+                }
+            }
         };
       if (wt == 0 && blockIdx.x < n_tiles && n_chunks > 0)
         load_b (0);
@@ -241,55 +286,34 @@ k_stft_mags_tc (const float *__restrict__ pcm, long long n_frames, int C, int n_
             }
           for (int c = 0; c < n_chunks; c++, g++)
             {
+              float d[kTcN / 2];
+#pragma unroll
+              for (int i = 0; i < kTcN / 2; i++)
+                d[i] = 0.f;
               mbar_wait_relaxed (b_full, g & 1);
-              for (int blk = 0; blk < 2 * (kTcN / kTcNB); blk++)
+              uint32_t a_base = a_addr;
+              asm volatile ("" : "+r"(a_base));
+              const uint64_t da = smem_desc_kmajor (a_base, kTcTile * 16, 128), db = smem_desc_kmajor (b_addr, kTcN * 16, 128);
+              wgmma_fence();
+              mma_half (d, da, db, 0);
+              wgmma_wait<0>();
+              store_half (d, shift_idx, f0, c, 0);
+              wgmma_fence();
+              mma_half (d, da, db, 1);
+              wgmma_wait<0>();
+              // every wgmma of the chunk has retired: this warp no longer reads A (last chunk) or B
+              __syncwarp();
+              if (c == n_chunks - 1 && lane == 0)
+                mbar_arrive (&a_empty[a]);
+              asm volatile ("bar.sync 1, %0;" :: "n"(kTcEpiWarps * 32) : "memory");      // the whole warpgroup is past B
+              if (wt == 0)
                 {
-                  const int mh = blk / (kTcN / kTcNB), nb = blk % (kTcN / kTcNB);
-                  float d[16];
-#pragma unroll
-                  for (int i = 0; i < 16; i++)
-                    d[i] = 0.f;
-                  wgmma_fence();
-#pragma unroll
-                  for (int sp = 0; sp < 2; sp++)
-#pragma unroll
-                    for (int j = 0; j < kTcK / 16; j++)
-                      wgmma_m64n32k16_f16 (d, smem_desc_kmajor (a_addr + sp * kTcASplit + j * 2 * (kTcTile * 16) + mh * (64 / 8) * 128, kTcTile * 16, 128),
-                                           smem_desc_kmajor (b_addr + j * 2 * (kTcN * 16) + nb * (kTcNB / 8) * 128, kTcN * 16, 128), (sp | j) != 0);
-                  wgmma_commit();
-                  wgmma_wait_all();
-#pragma unroll
-                  for (int i = 0; i < 16; i++)
-                    wgmma_fence_operand (d[i]);
-                  if (blk == 2 * (kTcN / kTcNB) - 1)
-                    {
-                      // the last block of the chunk has been computed: this warp no longer reads A (last chunk) or B
-                      __syncwarp();
-                      if (c == n_chunks - 1 && lane == 0)
-                        mbar_arrive (&a_empty[a]);
-                      asm volatile ("bar.sync 1, %0;" :: "n"(kTcEpiWarps * 32) : "memory");      // the whole warpgroup is past B
-                      if (wt == 0)
-                        {
-                          if (c + 1 < n_chunks)
-                            load_b (c + 1);
-                          else if (t + int (gridDim.x) < n_tiles)
-                            load_b (0);
-                        }
-                    }
-                  const int e_base = c * kTcChunkEnt + nb * (kTcNB / 2) + (lane & 3);
-                  const int f = f0 + mh * 64 + wi * 16 + (lane >> 2);           // f + 8 < ld always (ld multiple of 128)
-#pragma unroll
-                  for (int q = 0; q < kTcNB / 8; q++)
-                    {
-                      const int e = e_base + 4 * q;
-                      if (e < n_ent)
-                        {
-                          float2 *row = mags + ((size_t) shift_idx * n_ent + e) * ld + f;
-                          row[0] = make_float2 (d[4 * q], d[4 * q + 1]);
-                          row[8] = make_float2 (d[4 * q + 2], d[4 * q + 3]);
-                        }
-                    }
+                  if (c + 1 < n_chunks)
+                    load_b (c + 1);
+                  else if (t + int (gridDim.x) < n_tiles)
+                    load_b (0);
                 }
+              store_half (d, shift_idx, f0, c, 1);
             }
         }
     }

@@ -76,20 +76,28 @@ __device__ __forceinline__ uint64_t smem_desc_kmajor (uint32_t smem_addr, uint32
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile ("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile ("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile ("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most `Pending` committed wgmma groups of this thread are still in flight
+template <int Pending>
+__device__ __forceinline__ void wgmma_wait() { asm volatile ("wgmma.wait_group.sync.aligned %0;" :: "n"(Pending) : "memory"); }
 // keeps the compiler from touching accumulator registers across the asynchronous MMA (reads after the wait stay after it)
 __device__ __forceinline__ void wgmma_fence_operand (float& r) { asm volatile ("" : "+f"(r) :: "memory"); }
 
-// D (+)= A[smem] * B[smem]^T for a 64 x 32 tile, K = 16, fp16 inputs, fp32 accumulators; the whole warpgroup (4 aligned warps)
+// D (+)= A[smem] * B[smem]^T for a 64 x 96 tile, K = 16, fp16 inputs, fp32 accumulators; the whole warpgroup (4 aligned warps)
 // issues it together.  Accumulator fragment of thread t (warp wi = t / 32, lane l): d[4 q + 2 h + c] holds row 16 wi + l / 4 + 8 h,
 // column 8 q + 2 (l % 4) + c.
-__device__ __forceinline__ void wgmma_m64n32k16_f16 (float (&d)[16], uint64_t desc_a, uint64_t desc_b, bool accumulate)
+__device__ __forceinline__ void wgmma_m64n96k16_f16 (float (&d)[48], uint64_t desc_a, uint64_t desc_b, bool accumulate)
 {
-  asm volatile ("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-                "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+  asm volatile ("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+                "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
+                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+                "%48, %49, p, 1, 1, 0, 0;\n\t}"
                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                  "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                  "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
                 : "l"(desc_a), "l"(desc_b), "r"(accumulate ? 1u : 0u) : "memory");
 }
 
