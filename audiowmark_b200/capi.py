@@ -29,8 +29,8 @@ EXPORTS = [
     "awm_create", "awm_destroy", "awm_last_error", "awm_launch_count", "awm_stream", "awm_synchronize",
     "awm_profile_enable", "awm_profile_report", "awm_host_alloc", "awm_host_free",
     "awm_fft_r2c", "awm_fft_c2r", "awm_set_embed_tables", "awm_set_sync_tables", "awm_set_mix_tables",
-    "awm_pcm_bind", "awm_pcm_prefetch", "awm_embed", "awm_sync_approx", "awm_sync_approx_enqueue", "awm_sync_use_slot", "awm_sync_have", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_sync_refine_rescored", "awm_decode_blocks", "awm_viterbi",
-    "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_copy", "awm_is_device_pointer", "awm_speed_scan", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_prefetch_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
+    "awm_pcm_bind", "awm_embed", "awm_sync_approx", "awm_sync_approx_enqueue", "awm_sync_use_slot", "awm_sync_have", "awm_sync_peaks", "awm_sync_refine", "awm_sync_refine_offsets", "awm_sync_refine_rescored", "awm_decode_blocks", "awm_viterbi",
+    "awm_resample", "awm_pcm_push_resampled", "awm_pcm_pop", "awm_copy_to_host", "awm_copy", "awm_is_device_pointer", "awm_speed_scan", "awm_gather", "awm_pcm_bind_s16", "awm_pcm_device", "awm_embed_s16", "awm_embed_window", "awm_pcm_stage", "awm_pcm_stage_wait", "awm_dist_unique_id", "awm_dist_init", "awm_dist_world", "awm_dist_allgather",
     "awm_set_embed_roles", "awm_batch_validate", "awm_embed_batch", "awm_batch_rates_validate", "awm_embed_batch_rates",
     "awm_batch_offsets_validate", "awm_embed_batch_offsets", "awm_batch_rates_offsets_validate", "awm_embed_batch_rates_offsets",
     "awm_set_embed_roles_keys", "awm_get_embed_roles_keys", "awm_batch_keys_validate", "awm_embed_batch_keys",

@@ -164,9 +164,6 @@ struct awm_ctx
   // bound PCM
   const float *pcm = nullptr; size_t pcm_frames = 0; int pcm_ch = 0;
   DevBuf pcm_own, pcm16_own;
-  struct Prefetch { DevBuf buf, buf16; bool s16 = false; const void *src = nullptr; size_t n_frames = 0; int ch = 0; cudaEvent_t done = nullptr; bool valid = false; };   // s16: buf16 holds the copy, it becomes float in buf when it is bound
-  Prefetch pref[2];
-  int pref_next = 0;
   /* awm_pcm_stage: a host stream on its way into `staged` piece by piece */
   DevBuf staged, staged16;
   std::vector<cudaEvent_t> stage_done;           // one per piece, recorded on s_in
@@ -389,7 +386,7 @@ awm_destroy (awm_ctx *ctx)
   cudaStreamSynchronize (ctx->stream);
   if (ctx->s_approx)
     cudaStreamSynchronize (ctx->s_approx);
-  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->key_roles, &ctx->keygen_keys, &ctx->keygen_j, &ctx->keygen_ud, &ctx->keygen_idx, &ctx->keygen_err, &ctx->rate_items, &ctx->rate_scratch, &ctx->pcm_own, &ctx->pcm16_own, &ctx->dbT, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
+  DevBuf *bufs[] = { &ctx->tw, &ctx->win, &ctx->synth, &ctx->frame_mod, &ctx->roles, &ctx->batch_items, &ctx->batch_coded, &ctx->key_roles, &ctx->keygen_keys, &ctx->keygen_j, &ctx->keygen_ud, &ctx->keygen_idx, &ctx->keygen_err, &ctx->rate_items, &ctx->rate_scratch, &ctx->pcm_own, &ctx->pcm16_own, &ctx->staged, &ctx->staged16, &ctx->dbT, &ctx->peaks_out, &ctx->peaks_cnt, &ctx->a_mags,
                      &ctx->cand_start, &ctx->cand_noff, &ctx->r_ud, &ctx->r_cnt, &ctx->rvalid, &ctx->r_ent_ud, &ctx->r_ent_flag, &ctx->tw1024,
                      &ctx->cand_score, &ctx->rank_keep, &ctx->rank_first, &ctx->ex_start, &ctx->ex_cand, &ctx->ex_off, &ctx->ex_n, &ctx->vit_off, &ctx->blk_start, &ctx->D, &ctx->raw,
                      &ctx->vit_raw, &ctx->vit_types, &ctx->vit_delta, &ctx->vit_dec, &ctx->vit_bits, &ctx->vit_err,
@@ -406,13 +403,6 @@ awm_destroy (awm_ctx *ctx)
     nccl_destroy (ctx->nccl_comm);
   for (auto& ct : ctx->coef_cache)
     ct.second.buf.release();
-  for (auto& pf : ctx->pref)
-    {
-      pf.buf.release();
-      pf.buf16.release();
-      if (pf.done)
-        cudaEventDestroy (pf.done);
-    }
   for (KeyTab& k : ctx->keys)
     {
       for (SyncTab& s : k.sync)
@@ -831,25 +821,7 @@ pcm_bind_any (awm_ctx *ctx, const void *pcm_v, bool s16, size_t n_frames, int ch
   ctx->pushed = false;                           // a new bind replaces whatever awm_pcm_push_resampled saved
   const float *pcm = s16 ? nullptr : static_cast<const float *> (pcm_v);
   const bool dev = pcm_v && is_device_ptr (pcm_v);
-  awm_ctx::Prefetch *hit = nullptr;
-  if (!dev && pad_start == 0 && pad_end == 0)
-    for (auto& pf : ctx->pref)
-      if (pf.valid && pf.src == pcm_v && pf.n_frames == n_frames && pf.ch == channels && pf.s16 == s16)
-        hit = &pf;
-  if (hit)
-    {
-      CK (cudaStreamWaitEvent (ctx->stream, hit->done, 0));   // the prefetched copy becomes the bound PCM
-      if (hit->s16)
-        {
-          const long long n_val = (long long) (n_frames * channels);
-          PROF (ctx);
-          s16_to_f32_kernel (hit->buf16.as<int16_t>(), hit->buf.as<float>())<<<unsigned (((n_val + 1) / 2 + 255) / 256), 256, 0, ctx->stream>>> (hit->buf16.as<int16_t>(), hit->buf.as<float>(), n_val);
-          LAUNCH_CHECK ("k_s16_to_f32");
-        }
-      ctx->pcm = hit->buf.as<float>();
-      hit->valid = false;
-    }
-  else if (dev && !s16 && pad_start == 0 && pad_end == 0)
+  if (dev && !s16 && pad_start == 0 && pad_end == 0)
     {
       ctx->pcm = pcm;
     }
@@ -886,75 +858,10 @@ pcm_bind_any (awm_ctx *ctx, const void *pcm_v, bool s16, size_t n_frames, int ch
   return 0;
 }
 
-int
-pcm_prefetch_any (awm_ctx *ctx, const void *pcm, bool s16, size_t n_frames, int channels)
-{
-  if (!pcm || !n_frames || channels <= 0)
-    return fail (ctx, "awm_pcm_prefetch: bad arguments");
-  CK (cudaSetDevice (ctx->device));
-  if (is_device_ptr (pcm))
-    return 0;                                     // nothing to do: device memory is bound in place
-  if (!ctx->s_in)
-    {
-      CK (cudaStreamCreateWithFlags (&ctx->s_in, cudaStreamNonBlocking));
-      CK (cudaStreamCreateWithFlags (&ctx->s_out, cudaStreamNonBlocking));
-    }
-  awm_ctx::Prefetch& pf = ctx->pref[ctx->pref_next];
-  /* the slot's previous contents may still be the bound PCM of kernels in flight: order the copy behind them */
-  cudaEvent_t busy;
-  CK (cudaEventCreateWithFlags (&busy, cudaEventDisableTiming));
-  CK (cudaEventRecord (busy, ctx->stream));
-  CK (cudaStreamWaitEvent (ctx->s_in, busy, 0));
-  CK (cudaEventDestroy (busy));
-  if (ctx->pcm == pf.buf.p)
-    ctx->pcm_ch = 0;                              // the bound PCM is about to be overwritten: force a new bind
-  const size_t n_val = n_frames * channels;
-  CK (pf.buf.reserve (n_val * sizeof (float)));
-  if (!pf.done)
-    CK (cudaEventCreateWithFlags (&pf.done, cudaEventDisableTiming));
-  /* Consecutive chunks of `get` overlap (WavChunkLoader: 134 s of 30 min).  When this span starts inside the span that was prefetched
-   * just before it and is still waiting to be bound, its head is already on the device: it is copied from there (device to device,
-   * ordered behind that upload on the same stream) and only the rest crosses PCIe -- 7 % fewer bytes for a 1 h stream. */
-  size_t head = 0;                              // frames taken from the previous prefetch
-  if (s16)
-    CK (pf.buf16.reserve (n_val * sizeof (int16_t)));
-  {
-    awm_ctx::Prefetch& prev = ctx->pref[ctx->pref_next ^ 1];
-    const size_t esz = (s16 ? sizeof (int16_t) : sizeof (float)) * size_t (channels);
-    const char *b0 = static_cast<const char *> (prev.src), *p0 = static_cast<const char *> (pcm);
-    if (prev.valid && prev.s16 == s16 && prev.ch == channels && b0 && p0 > b0 && p0 < b0 + prev.n_frames * esz && size_t (p0 - b0) % esz == 0)
-      {
-        const size_t first = size_t (p0 - b0) / esz;
-        head = std::min (prev.n_frames - first, n_frames);
-        if (s16)            // 16 bit audio stays 16 bit until it is bound (see below)
-          CK (cudaMemcpyAsync (pf.buf16.p, prev.buf16.as<int16_t>() + first * channels, head * channels * sizeof (int16_t), cudaMemcpyDeviceToDevice, ctx->s_in));
-        else
-          CK (cudaMemcpyAsync (pf.buf.p, prev.buf.as<float>() + first * channels, head * channels * sizeof (float), cudaMemcpyDeviceToDevice, ctx->s_in));
-      }
-  }
-  /* the copy stream carries copies only: the int -> float conversion of 16 bit audio runs on the context stream when the chunk is
-   * bound (pcm_bind_any), so the copy of the next chunk starts the moment this one has arrived */
-  const size_t rest = (n_frames - head) * channels, head_val = head * channels;
-  if (rest && s16)
-    CK (cudaMemcpyAsync (pf.buf16.as<int16_t>() + head_val, static_cast<const int16_t *> (pcm) + head_val, rest * sizeof (int16_t), cudaMemcpyHostToDevice, ctx->s_in));
-  else if (rest)
-    CK (cudaMemcpyAsync (pf.buf.as<float>() + head_val, static_cast<const float *> (pcm) + head_val, rest * sizeof (float), cudaMemcpyHostToDevice, ctx->s_in));
-  CK (cudaEventRecord (pf.done, ctx->s_in));
-  pf.src = pcm;
-  pf.n_frames = n_frames;
-  pf.ch = channels;
-  pf.s16 = s16;
-  pf.valid = true;
-  ctx->pref_next ^= 1;
-  return 0;
-}
-
 } // namespace
 
 int awm_pcm_bind (awm_ctx *ctx, const float *pcm, size_t n_frames, int channels, size_t pad_start, size_t pad_end) { return pcm_bind_any (ctx, pcm, false, n_frames, channels, pad_start, pad_end); }
 int awm_pcm_bind_s16 (awm_ctx *ctx, const int16_t *pcm, size_t n_frames, int channels, size_t pad_start, size_t pad_end) { return pcm_bind_any (ctx, pcm, true, n_frames, channels, pad_start, pad_end); }
-int awm_pcm_prefetch (awm_ctx *ctx, const float *pcm, size_t n_frames, int channels) { return pcm_prefetch_any (ctx, pcm, false, n_frames, channels); }
-int awm_pcm_prefetch_s16 (awm_ctx *ctx, const int16_t *pcm, size_t n_frames, int channels) { return pcm_prefetch_any (ctx, pcm, true, n_frames, channels); }
 
 /* awm_pcm_stage / awm_pcm_stage_wait: see include/awm_b200.h */
 int
@@ -1768,8 +1675,8 @@ awm_sync_approx_enqueue (awm_ctx *ctx, int slot, int key_slot, int mode, uint64_
   if (slot < 0 || slot > 1)
     return fail (ctx, "awm_sync_approx_enqueue: bad slot %d", slot);
   /* the slot keeps a pointer to the bound PCM until it is used: a buffer of the context would be overwritten by the next bind or
-   * prefetch in the meantime */
-  const void *own[] = { ctx->pcm_own.p, ctx->pref[0].buf.p, ctx->pref[1].buf.p, ctx->staged.p, ctx->pcm_rs.p };
+   * stage in the meantime */
+  const void *own[] = { ctx->pcm_own.p, ctx->staged.p, ctx->pcm_rs.p };
   for (const void *b : own)
     if (b && ctx->pcm == b)
       return fail (ctx, "awm_sync_approx_enqueue: the bound PCM must be the caller's device memory, not a buffer of the context");

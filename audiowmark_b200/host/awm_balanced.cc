@@ -281,8 +281,7 @@ Get::Get (int rank, int world, size_t n_total, const float *pcm, const int16_t *
     m_dev = pcm;
   else
     {
-      const size_t piece = size_t (8) << 20;                       // sample-frames per piece (32 MB of 16 bit stereo)
-      if (awm_pcm_stage (ctx, pcm16 ? static_cast<const void *> (pcm16) : pcm, pcm16 ? 1 : 0, pcm_frames, channels, piece, &m_dev))
+      if (awm_pcm_stage (ctx, pcm16 ? static_cast<const void *> (pcm16) : pcm, pcm16 ? 1 : 0, pcm_frames, channels, kStagePiece, &m_dev))
         {
           error ("audiowmark: %s\n", awm_last_error (ctx));
           return;

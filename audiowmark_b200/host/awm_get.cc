@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <math.h>
 #include <string.h>
 #include <stdlib.h>
@@ -397,64 +398,33 @@ public:
   }
 };
 
-/* the audio of a chunk: float samples (host or device memory) or 16 bit PCM in host memory, which is converted on the device
- * (awm_pcm_bind_s16) so that only half the bytes cross PCIe */
-struct PcmRef
-{
-  const float   *f32 = nullptr;
-  const int16_t *s16 = nullptr;
-  PcmRef advanced (size_t values) const { PcmRef r; r.f32 = f32 ? f32 + values : nullptr; r.s16 = s16 ? s16 + values : nullptr; return r; }
-  int bind (awm_ctx *ctx, size_t n_frames, int n_channels) const
-  {
-    return s16 ? awm_pcm_bind_s16 (ctx, s16, n_frames, n_channels, 0, 0) : awm_pcm_bind (ctx, f32, n_frames, n_channels, 0, 0);
-  }
-  int prefetch (awm_ctx *ctx, size_t n_frames, int n_channels) const
-  {
-    return s16 ? awm_pcm_prefetch_s16 (ctx, s16, n_frames, n_channels) : awm_pcm_prefetch (ctx, f32, n_frames, n_channels);
-  }
-  /* float samples in host memory (what the clip decoder cuts and pads): only needed for short inputs */
-  const float *host_floats (awm_ctx *ctx, size_t n_values, vector<float>& storage) const
-  {
-    if (s16)
-      {
-        storage.resize (n_values);
-        const float norm = 1.0 / 0x80000000LL;                 /* src/sfinputstream.cc:207-209 */
-        for (size_t i = 0; i < n_values; i++)
-          storage[i] = (int (s16[i]) << 16) * norm;
-        return storage.data();
-      }
-    if (Engine::is_device_pointer (f32))
-      {
-        storage.resize (n_values);
-        if (awm_copy_to_host (ctx, storage.data(), f32, n_values * sizeof (float)))
-          return nullptr;
-        return storage.data();
-      }
-    return f32;
-  }
-};
-
 /* decode (src/wmget.cc:886-939) for one chunk: everything up to the soft bits; the Viterbi jobs are queued.
+ * pcm: the chunk's float samples in device memory, bound in place.  host_pcm (optional): the same samples in host memory; else the
+ * clip decoder, which cuts and pads on the host, copies them back (short inputs only).
  * approx_slot >= 0: one key, no speed detection; the chunk's approx search has been queued into that slot (awm_sync_approx_enqueue) */
 int
-decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vector<Key>& key_list, const PcmRef& pcm, size_t n_frames,
-              int n_channels, int sample_rate, bool first_chunk, bool print_speed_results, int approx_slot)
+decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vector<Key>& key_list, const float *pcm, const float *host_pcm,
+              size_t n_frames, int n_channels, int sample_rate, bool first_chunk, bool print_speed_results, int approx_slot)
 {
   awm_ctx *ctx = Engine::ctx();
   if (!ctx)
     return 1;
-  if (approx_slot < 0 && pcm.bind (ctx, n_frames, n_channels))
+  if (approx_slot < 0 && awm_pcm_bind (ctx, pcm, n_frames, n_channels, 0, 0))
     {
       error ("audiowmark: %s\n", awm_last_error (ctx));
       return 1;
     }
   vector<float> host_storage;
-  const float *host_samples = nullptr;          /* fetched lazily: only the clip decoder needs it */
   auto need_host = [&] () -> const float *
     {
-      if (!host_samples)
-        host_samples = pcm.host_floats (ctx, n_frames * n_channels, host_storage);
-      return host_samples;
+      if (!host_pcm)
+        {
+          host_storage.resize (n_frames * n_channels);
+          if (awm_copy_to_host (ctx, host_storage.data(), pcm, host_storage.size() * sizeof (float)))
+            return nullptr;
+          host_pcm = host_storage.data();
+        }
+      return host_pcm;
     };
   /* The strategy for integrating speed detection into decoding (src/wmget.cc:888-928):
    *  - the watermark is always decoded on the original data
@@ -464,11 +434,7 @@ decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vect
     {
       vector<DetectSpeedResult> speed_results;
       if (Params::detect_speed || Params::detect_speed_patient)
-        {
-          /* 16 bit input: the float copy that was just bound on the device serves the speed scan as well */
-          const float *speed_samples = pcm.s16 ? awm_pcm_device (ctx, nullptr, nullptr) : pcm.f32;
-          speed_results = detect_speed (key_list, speed_samples, n_frames, n_channels, sample_rate, print_speed_results);
-        }
+        speed_results = detect_speed (key_list, pcm, n_frames, n_channels, sample_rate, print_speed_results);
       else
         for (const auto& key : key_list)
           speed_results.push_back ({ key, Params::try_speed });
@@ -478,7 +444,7 @@ decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vect
           /* resample_ratio (wav_data, speed, mark_sample_rate * speed): the stretched chunk stays on the device */
           const size_t speed_frames = lrint (double (n_frames) * speed_result.speed);
           const int speed_rate = Params::mark_sample_rate * speed_result.speed;
-          if (rebind && pcm.bind (ctx, n_frames, n_channels))
+          if (rebind && awm_pcm_bind (ctx, pcm, n_frames, n_channels, 0, 0))
             return 1;
           rebind = false;
           if (awm_pcm_push_resampled (ctx, speed_result.speed, 16, speed_frames))
@@ -500,7 +466,7 @@ decode_chunk (vector<VitJob>& pending, int chunk, string& debug_sync, const vect
               rebind = true;
             }
         }
-      if (rebind && pcm.bind (ctx, n_frames, n_channels))
+      if (rebind && awm_pcm_bind (ctx, pcm, n_frames, n_channels, 0, 0))
         return 1;
     }
   const double tb0 = get_time();
@@ -558,6 +524,28 @@ move_to_front (awm_ctx *ctx, float *buf, size_t from, size_t n, int channels)
       done += k;
     }
   return true;
+}
+
+/* the end of a `get`: one Viterbi launch over the jobs of all chunks, then the reference's per-chunk merge in chunk order */
+int
+merge_chunk_results (vector<VitJob>& pending, const vector<GetStream::Chunk>& chunks, const vector<string>& debug_syncs, const vector<Key>& key_list,
+                     ResultSet& result_set)
+{
+  vector<ResultSet> chunk_results (chunks.size());
+  const double tv0 = get_time();
+  const size_t n_jobs = pending.size();
+  if (!run_viterbi_jobs (pending, chunk_results))
+    return 1;
+  if (getenv ("AWM_TRACE"))
+    fprintf (stderr, "[trace] viterbi: %zu jobs %.3f ms\n", n_jobs, (get_time() - tv0) * 1e3);
+  for (size_t c = 0; c < chunk_results.size(); c++)
+    {
+      chunk_results[c].set_debug_sync (debug_syncs[c]);
+      chunk_results[c].apply_time_offset (chunks[c].time_offset);
+      result_set.merge (chunk_results[c]);
+    }
+  result_set.sort (key_list);
+  return 0;
 }
 
 }
@@ -637,13 +625,9 @@ GetStream::decode()
   const int chunk = int (m_chunks.size());
   m_chunks.push_back ({ m_start, m_fill, m_time_offset });
   string debug_sync;
-  if (!m_dry)
-    {
-      PcmRef pcm;
-      pcm.f32 = m_chunk;
-      if (decode_chunk (m_pending, chunk, debug_sync, m_keys, pcm, m_fill, m_channels, Params::mark_sample_rate, chunk == 0, m_print_speed, -1))
-        return false;
-    }
+  if (!m_dry && decode_chunk (m_pending, chunk, debug_sync, m_keys, m_chunk, nullptr, m_fill, m_channels, Params::mark_sample_rate, chunk == 0,
+                              m_print_speed, -1))
+    return false;
   m_debug_syncs.push_back (debug_sync);
   return true;
 }
@@ -772,18 +756,7 @@ GetStream::finish (ResultSet& result_set, size_t *mark_rate_frames)
     *mark_rate_frames = m_produced;
   if (m_dry || m_chunks.empty())
     return 0;
-  /* one Viterbi launch, then the reference's per-chunk merge in chunk order */
-  vector<ResultSet> chunk_results (m_chunks.size());
-  if (!run_viterbi_jobs (m_pending, chunk_results))
-    return 1;
-  for (size_t c = 0; c < chunk_results.size(); c++)
-    {
-      chunk_results[c].set_debug_sync (m_debug_syncs[c]);
-      chunk_results[c].apply_time_offset (m_chunks[c].time_offset);
-      result_set.merge (chunk_results[c]);
-    }
-  result_set.sort (m_keys);
-  return 0;
+  return merge_chunk_results (m_pending, m_chunks, m_debug_syncs, m_keys, result_set);
 }
 
 int
@@ -829,31 +802,36 @@ get_watermark_pcm (const vector<Key>& key_list, const float *samples, const int1
   chunk_geometry (sample_rate, max_frames, overlap);
   size_t start = 0, end = min (max_frames, n_frames);
   double time_offset = 0;
-  bool first_chunk = true, eof = end < max_frames;
+  bool eof = end < max_frames;
   if (n_frames == 0)
     return 0;
   /* pass 1: sync search + soft bits per chunk (GPU), Viterbi jobs of all chunks are collected */
   vector<VitJob> pending;
-  vector<double> time_offsets;
+  vector<GetStream::Chunk> chunks;
   vector<string> debug_syncs;
   awm_ctx *ctx = Engine::ctx();
   if (!ctx)
     return 1;
-  /* host buffers: the next chunk travels over PCIe while the current one is searched */
-  PcmRef pcm;
-  pcm.f32 = samples16 ? nullptr : samples;
-  pcm.s16 = samples16;
-  pcm.prefetch (ctx, end - start, n_channels);
+  /* host input crosses PCIe once, piece by piece: a chunk waits only for the pieces it reads, so the later chunks travel while the
+   * first one is searched.  Device float input is bound in place. */
+  const bool staged = samples16 || !Engine::is_device_pointer (samples);
+  const float *pcm = samples;
+  if (staged && awm_pcm_stage (ctx, samples16 ? static_cast<const void *> (samples16) : samples, samples16 ? 1 : 0, n_frames, n_channels,
+                               kStagePiece, &pcm))
+    {
+      error ("audiowmark: %s\n", awm_last_error (ctx));
+      return 1;
+    }
+  const float *host_pcm = staged && !samples16 ? samples : nullptr;
   /* Device PCM of several chunks, one key, no speed detection: the approx search of chunk k + 1 is queued (on a second stream, into
    * the other approx slot) before chunk k's candidate selection, refine and decode, so that the GPU has work while the host makes
    * those decisions.  Every decision still runs per chunk, in the same order, on the same values.  Host PCM keeps the serial loop:
-   * there the next chunk's upload, not the GPU, sets the pace. */
+   * there the upload, not the GPU, sets the pace. */
   const bool speed = Params::detect_speed || Params::detect_speed_patient || Params::try_speed > 0;
-  const int pipe_key = (!eof && key_list.size() == 1 && !speed && !Params::test_no_sync && pcm.f32 && Engine::is_device_pointer (pcm.f32))
-                       ? Engine::key_slot (key_list[0]) : -1;
+  const int pipe_key = (!eof && key_list.size() == 1 && !speed && !Params::test_no_sync && !staged) ? Engine::key_slot (key_list[0]) : -1;
   auto enqueue_approx = [&] (size_t c0, size_t c1, int approx_slot)
     {
-      if (pcm.advanced (c0 * n_channels).bind (ctx, c1 - c0, n_channels)
+      if (awm_pcm_bind (ctx, pcm + c0 * n_channels, c1 - c0, n_channels, 0, 0)
           || awm_sync_approx_enqueue (ctx, approx_slot, pipe_key, AWM_MODE_BLOCK, 0, (c1 - c0) * n_channels, Params::water_delta))
         {
           error ("audiowmark: %s\n", awm_last_error (ctx));
@@ -863,25 +841,51 @@ get_watermark_pcm (const vector<Key>& key_list, const float *samples, const int1
     };
   if (pipe_key >= 0 && !enqueue_approx (start, end, 0))
     return 1;
+  std::unique_ptr<void, void (*) (void *)> aligned_chunk (nullptr, [] (void *p) { awm_device_free (Engine::ctx(), p); });
   for (;;)
     {
       string debug_sync;
-      const int chunk = int (time_offsets.size());
-      if (!eof)
+      const int chunk = int (chunks.size());
+      if (!eof && pipe_key >= 0)
         {
           const size_t nstart = end - overlap, nend = min (nstart + max_frames, n_frames);
-          pcm.advanced (nstart * n_channels).prefetch (ctx, nend - nstart, n_channels);
-          if (pipe_key >= 0 && !enqueue_approx (nstart, nend, (chunk + 1) & 1))
+          if (!enqueue_approx (nstart, nend, (chunk + 1) & 1))
             return 1;
-          if (pipe_key >= 0 && getenv ("AWM_TRACE"))
+          if (getenv ("AWM_TRACE"))
             fprintf (stderr, "[trace] chunk %d: approx search of chunk %d queued ahead\n", chunk, chunk + 1);
         }
-      if (decode_chunk (pending, chunk, debug_sync, key_list, pcm.advanced (start * n_channels), end - start, n_channels, sample_rate, first_chunk,
-                        print_speed_results, pipe_key >= 0 ? chunk & 1 : -1))
+      if (staged && awm_pcm_stage_wait (ctx, end))
+        {
+          error ("audiowmark: %s\n", awm_last_error (ctx));
+          return 1;
+        }
+      const float *chunk_pcm = pcm + start * n_channels;
+      /* The sync search reads stereo PCM at a 16-byte aligned address by bulk copies and at any other by global loads, whose sums
+       * can differ in the last bits.  A staged chunk that starts at an odd frame (an odd chunk step, as with --frames-per-bit 3) is
+       * searched from an aligned copy, so that a host `get` finds what GetStream finds, which searches every chunk from the start
+       * of its own buffer. */
+      if (staged && n_channels == 2 && (reinterpret_cast<uintptr_t> (chunk_pcm) & 15))
+        {
+          void *buf = nullptr;
+          if (!aligned_chunk && awm_device_alloc (ctx, max_frames * n_channels * sizeof (float), &buf))
+            {
+              error ("audiowmark: %s\n", awm_last_error (ctx));
+              return 1;
+            }
+          if (buf)
+            aligned_chunk.reset (buf);
+          if (awm_copy (ctx, aligned_chunk.get(), chunk_pcm, (end - start) * n_channels * sizeof (float)))
+            {
+              error ("audiowmark: %s\n", awm_last_error (ctx));
+              return 1;
+            }
+          chunk_pcm = static_cast<const float *> (aligned_chunk.get());
+        }
+      if (decode_chunk (pending, chunk, debug_sync, key_list, chunk_pcm, host_pcm ? host_pcm + start * n_channels : nullptr, end - start,
+                        n_channels, sample_rate, chunk == 0, print_speed_results, pipe_key >= 0 ? chunk & 1 : -1))
         return 1;
-      time_offsets.push_back (time_offset);
+      chunks.push_back ({ start, end - start, time_offset });
       debug_syncs.push_back (debug_sync);
-      first_chunk = false;
       if (eof)
         break;
       time_offset += double (end - start - overlap) / sample_rate;
@@ -890,22 +894,7 @@ get_watermark_pcm (const vector<Key>& key_list, const float *samples, const int1
       eof = (new_end - start) < max_frames;
       end = new_end;
     }
-  /* pass 2: one Viterbi launch, then the reference's per-chunk merge in chunk order */
-  vector<ResultSet> chunk_results (time_offsets.size());
-  const double tv0 = get_time();
-  const size_t n_jobs = pending.size();
-  if (!run_viterbi_jobs (pending, chunk_results))
-    return 1;
-  if (getenv ("AWM_TRACE"))
-    fprintf (stderr, "[trace] viterbi: %zu jobs %.3f ms\n", n_jobs, (get_time() - tv0) * 1e3);
-  for (size_t c = 0; c < chunk_results.size(); c++)
-    {
-      chunk_results[c].set_debug_sync (debug_syncs[c]);
-      chunk_results[c].apply_time_offset (time_offsets[c]);
-      result_set.merge (chunk_results[c]);
-    }
-  result_set.sort (key_list);
-  return 0;
+  return merge_chunk_results (pending, chunks, debug_syncs, key_list, result_set);
 }
 
 static int

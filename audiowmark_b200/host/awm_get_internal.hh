@@ -5,6 +5,9 @@
 
 namespace get_detail {
 
+/* sample-frames per piece of a host upload (awm_pcm_stage), 32 MB of 16 bit stereo: a chunk waits only for the pieces it reads */
+constexpr size_t kStagePiece = size_t (8) << 20;
+
 /* one code word waiting for the Viterbi decoder */
 struct VitJob
 {

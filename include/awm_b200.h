@@ -110,24 +110,20 @@ int awm_set_mix_tables (awm_ctx *ctx, int key_slot, const awm_mix_entry *entries
  * (ClipDecoder::run_block zero padding, src/wmget.cc:823-866) without the caller materialising them.
  */
 int awm_pcm_bind (awm_ctx *ctx, const float *pcm, size_t n_frames, int channels, size_t pad_start, size_t pad_end);
-/* optional: start copying a HOST buffer that will be bound next (the following chunk of a long file) on a separate
- * stream while the kernels of the current chunk run; a later awm_pcm_bind with the same pointer / size / channels and
- * no padding picks the copy up instead of transferring again.  Two prefetches may be outstanding.  A span that starts inside
- * the span prefetched just before it (the overlapping chunks of WavChunkLoader, src/wavchunkloader.cc:54-163) takes its head from
- * that device copy and only transfers the rest; the host memory of an unbound prefetch must not change meanwhile. */
-int awm_pcm_prefetch (awm_ctx *ctx, const float *pcm, size_t n_frames, int channels);
 
 /* 16 bit PCM variants: the buffers hold interleaved int16 (what a 16 bit WAV file holds); conversion to / from the float
  * pipeline happens on the device with the reference's rules -- reading: sample * 2^-15 (src/sfinputstream.cc:189-210),
  * writing: float_to_int_clip<32> (src/rawconverter.hh:34-50), 16 most significant bits kept (src/sfoutputstream.cc:148-155) --
  * so results are identical to converting on the host, at half the PCIe traffic. */
 int awm_pcm_bind_s16 (awm_ctx *ctx, const int16_t *pcm, size_t n_frames, int channels, size_t pad_start, size_t pad_end);
-int awm_pcm_prefetch_s16 (awm_ctx *ctx, const int16_t *pcm, size_t n_frames, int channels);
 /* A long HOST stream (float or 16 bit PCM) on its way to the device piece by piece, for callers that work on parts of it while the
- * rest is still crossing PCIe (the sharded get: a rank searches its first chunk slice while its later slices arrive; replaces the
- * read-ahead of WavChunkLoader, src/wavchunkloader.cc:54-163).  awm_pcm_stage starts the copies on a copy stream and returns the
- * device address of the float copy at once; awm_pcm_stage_wait (n) orders everything issued on the context stream afterwards
- * behind the arrival of the first n sample-frames.  Bind parts with awm_pcm_bind (device pointer + offset). */
+ * rest is still crossing PCIe; it replaces the read-ahead of WavChunkLoader (src/wavchunkloader.cc:54-163).  Both `get` drivers
+ * upload host input this way: get_watermark_buffer searches its first chunk while the later chunks arrive, and the sharded get
+ * searches a rank's first chunk slice while its later slices arrive.  awm_pcm_stage starts the copies on a copy stream and
+ * returns the device address of the float copy at once; awm_pcm_stage_wait (n) orders everything issued on the context stream
+ * afterwards behind the arrival of the first n sample-frames (16 bit pieces become float on the context stream then).  Bind
+ * parts with awm_pcm_bind (device pointer + offset).  A new stage reuses the buffer: parts of the previous one must not be read
+ * after it. */
 int awm_pcm_stage (awm_ctx *ctx, const void *pcm, int is_s16, size_t n_frames, int channels, size_t piece_frames, const float **device_out);
 int awm_pcm_stage_wait (awm_ctx *ctx, size_t n_frames);
 /* device copy (float) of the bound PCM incl. padding; NULL if nothing is bound */

@@ -165,7 +165,7 @@ def test_short_payload_and_linear_vs_reference(name):
 
 
 def test_s16_entry_points_equal_host_side_conversion():
-    """16 bit PCM buffers converted on the device (awm_embed_s16 / awm_pcm_bind_s16): bit identical to converting on the host
+    """16 bit PCM buffers converted on the device (awm_embed_s16 / awm_pcm_stage): bit identical to converting on the host
     with the reference's rules (src/sfinputstream.cc:189-210, src/rawconverter.hh:34-50 + src/sfoutputstream.cc:148-155) around
     the float entry points, for add (incl. clipping at full scale), get (block and clip decoder) and get --detect-speed"""
     H.set_params()

@@ -5,6 +5,7 @@ import json
 import numpy as np
 import pytest
 
+import awm_oracle as O
 import awm_testlib as T
 from audiowmark_b200 import hostapi as H, sharding as S
 
@@ -24,8 +25,9 @@ def test_sharded_embed_is_bit_identical():
 
 
 def test_pipelined_host_paths_equal_device_paths():
-    """awm_embed splits long HOST buffers into pieces to overlap H2D / kernels / D2H, and `get` prefetches the next chunk:
-    both must give exactly what the one-shot device-pointer path gives."""
+    """awm_embed splits long HOST buffers into pieces to overlap H2D / kernels / D2H, and `get` stages its whole input piece by piece
+    (awm_pcm_stage) and binds each chunk's slice once its pieces have arrived: both must give exactly what the one-shot device-pointer
+    path gives."""
     torch = pytest.importorskip("torch")
     x = T.noise(600.0, 2, seed=23, amp=1.0)                 # 10 min: three pieces of 12288 frames, limiter active
     H.set_params(chunk_size_min=4.0)
@@ -45,6 +47,48 @@ def test_pipelined_host_paths_equal_device_paths():
     assert H.get(want) == doc_dev
     H.set_params()
 
+
+
+def test_host_gets_back_to_back_read_only_their_own_upload():
+    """two host `get`s in a row on one context, the second on a shorter buffer, each over several chunks: every upload replaces the
+    staged stream (16 bit pieces are converted again), so each document equals the device-pointer `get` of the same audio"""
+    torch = pytest.importorskip("torch")
+    H.set_params(chunk_size_min=4.0)
+    try:
+        audio = [O.quantize_sndfile16(H.add(T.noise(seconds, 2, seed=seed), T.PAYLOAD)) for seconds, seed in ((600.0, 31), (380.0, 32))]
+        want = []
+        for y16 in audio:
+            yd = torch.from_numpy(O.int16_to_float(y16)).cuda()
+            torch.cuda.synchronize()
+            want.append(H.get(yd.data_ptr(), n_frames=y16.shape[0], channels=2))
+            assert any(m["bits"] == T.PAYLOAD for m in want[-1]["matches"])
+        assert [H.get(O.int16_to_float(y16)) for y16 in audio] == want
+        assert [H.get_s16(y16) for y16 in audio] == want
+    finally:
+        H.set_params()
+
+
+def test_try_speed_on_host_input_equals_device_input():
+    """--try-speed on host float and 16 bit input searches the staged device copy of each chunk, over several chunks and on a clip
+    short enough for the clip decoder, after which the chunk is bound again (here once per key): the documents equal the
+    device-input one"""
+    torch = pytest.importorskip("torch")
+    H.set_params(chunk_size_min=4.0)
+    H.set_speed_params(try_speed=T.cli_float(1.01))
+    try:
+        for seconds, keys in ((600.0, None), (100.0, [bytes(16), bytes(range(1, 17))])):
+            y = H.add(T.noise(seconds, 2, seed=33), T.PAYLOAD)
+            y16 = O.quantize_sndfile16(H.resample(y, 1 / T.cli_float(1.01)))
+            yf = O.int16_to_float(y16)
+            yd = torch.from_numpy(yf).cuda()
+            torch.cuda.synchronize()
+            want = H.get(yd.data_ptr(), keys=keys, n_frames=yf.shape[0], channels=2)
+            assert any(m["bits"] == T.PAYLOAD for m in want["matches"]), seconds
+            assert H.get(yf, keys=keys) == want
+            assert H.get_s16(y16, keys=keys) == want
+    finally:
+        H.set_speed_params()
+        H.set_params()
 
 @pytest.mark.parametrize("world", [1, 2, 3])
 def test_frame_balanced_get_equals_single_process(world):
