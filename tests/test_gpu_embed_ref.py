@@ -71,8 +71,9 @@ CEIL = float(np.float32(0.99))
 
 # ------------------------------------------------------------------------------------------------ float64 reference
 
-def _spectrum_delta(X, rows, wd, nz):
-    """D and its bound dD for one channel: X [F][101] complex, rows [F][101] table bytes, nz [F] windowed norm of the channel's pair"""
+def _spectrum_delta(X, rows, wd, nz, ex=0.0):
+    """D and its bound dD for one channel: X [F][101] complex, rows [F][101] table bytes, nz [F] windowed norm of the channel's pair,
+    ex [F] a bound of the error the input itself carries into every bin"""
     mag = np.abs(X)
     marked = rows != 0
     e = np.where(rows == 1, -wd, np.where(rows == 2, wd, 0.0))
@@ -84,7 +85,7 @@ def _spectrum_delta(X, rows, wd, nz):
         above = marked & (mag > MIN_MAG)
         Dfull = X * f
         D = np.where(above, Dfull, 0)
-        eX = (LAMBDA * (ETA * LOG2N + 2) * U * nz)[:, None]
+        eX = (LAMBDA * (ETA * LOG2N + 2) * U * nz + ex)[:, None]
         L2 = 2 * lmag / math.log(2)                                    # log2 of the power
         t = e * lmag / math.log(2)
         dt = np.abs(e) / 2 * (3 * U + 2 * U * np.abs(L2)) + 2 * U * np.abs(t)
@@ -95,10 +96,15 @@ def _spectrum_delta(X, rows, wd, nz):
     return D, np.where(np.isfinite(dD), dD, 0.0)
 
 
-def embed_ref(x, fm, frame_number0, wd=0.01, limiter_block=0, ceiling=CEIL, stream_pos0=0, snr_pos=(0, None), mutate=None, m0=1):
+def embed_ref(x, fm, frame_number0, wd=0.01, limiter_block=0, ceiling=CEIL, stream_pos0=0, snr_pos=(0, None), mutate=None, m0=1,
+              dx=None, delta_only=False):
     """float64 awm_embed of x [n][C] with FrameMod table fm [2][fpb][101]: (out [n][C], bound [n][C], (sum wm^2, sum x^2, bound of
-    the first)).  mutate: one of 'row', 'neighbour', 'peak', 'delta', 'swap' (test_bound_is_sharp), applied at frame / block m0."""
-    x = np.asarray(x, np.float32)
+    the first)).  mutate: one of 'row', 'neighbour', 'peak', 'delta', 'swap' (test_bound_is_sharp), applied at frame / block m0.
+    dx [n][C]: a bound of the error x itself carries (x is then a float64 value the GPU only approximates); it enters every bin of
+    channel c of frame m as sum_i WIN_i dx_c,i (the transform is linear, so an input error reaches its own channel's spectrum only;
+    the rounding the pair shares is the FFT term).  delta_only: the watermark signal alone (k_embed_batch's delta_only), n_proc * 1024
+    frames with the spill frame, no mix, no limiter."""
+    x = np.asarray(x, np.float64)
     n, C = x.shape
     if n == 0:
         return np.zeros((0, C)), np.zeros((0, C)), (0.0, 0.0, 0.0)
@@ -115,17 +121,22 @@ def embed_ref(x, fm, frame_number0, wd=0.01, limiter_block=0, ceiling=CEIL, stre
     rows = fm.reshape(2 * fpb, 101)[r]
     assert not rows[:, :P.min_band].any() and rows.max(initial=0) <= 2
     wd_used = wd * 1.01 if mutate == "delta" else wd
-    X, e2 = [], []
+    X, e2, ed = [], [], []
+    if dx is not None:
+        extd = np.zeros((n_real * N, C))
+        extd[:n] = dx
+        frd = extd.reshape(n_real, N, C)
     for c in range(C):
         xw = fr[:, :, c] * WIN
         e2.append((xw * xw).sum(axis=1))
         X.append(np.fft.rfft(xw, axis=1)[:, :101])
+        ed.append((frd[:, :, c] * WIN).sum(axis=1) if dx is not None else np.zeros(n_real))
     D, dD, nz = [], [], []
     for c in range(C):
         lo = c - c % 2
         nz.append(np.sqrt(e2[lo] + (e2[lo + 1] if lo + 1 < C else 0.0)))
         src = c ^ 1 if (mutate == "swap" and C >= 2 and c < 2) else c
-        d, b = _spectrum_delta(X[src], rows, wd_used, nz[c])
+        d, b = _spectrum_delta(X[src], rows, wd_used, nz[c], ed[c])
         D.append(d)
         dD.append(b)
     y = np.zeros((Ln, C))
@@ -151,38 +162,50 @@ def embed_ref(x, fm, frame_number0, wd=0.01, limiter_block=0, ceiling=CEIL, stre
         wm = ((t1 + t2) + t3).reshape(-1)
         bt = Ez[0:n_proc, None] * W2 + Ez[1:n_proc + 1, None] * W1 + Ez[2:n_proc + 2, None] * W0
         bwm = (bt + 3 * U * (np.abs(t1) + np.abs(t2) + np.abs(t3) + bt)).reshape(-1)
+        if delta_only:
+            y[:, c], by[:, c] = wm, bwm
+            continue
         y[:, c] = wm + ext[:, c]
         by[:, c] = bwm + np.where(np.abs(wm) + bwm > 0, U * (np.abs(y[:, c]) + bwm), 0.0)
         w = wm[p_lo:p_hi]
         snr_d += float((w * w).sum())
         snr_s += float((ext[p_lo:p_hi, c] ** 2).sum())
         snr_b += float((2 * np.abs(w) * bwm[p_lo:p_hi] + bwm[p_lo:p_hi] ** 2).sum())
+    if delta_only:
+        return y, by, None
     out, bound = y, by
     if limiter_block > 0:
-        B = limiter_block
-        g = stream_pos0 + np.arange(Ln, dtype=np.int64)
-        rel = g // B - stream_pos0 // B
-        starts = np.concatenate([[0], np.flatnonzero(np.diff(rel)) + 1])
-        pk = np.maximum.reduceat(np.abs(y).max(axis=1), starts)
-        dpk = np.maximum.reduceat(by.max(axis=1), starts)
-        if mutate == "peak" and m0 + 1 < len(pk):
-            pk[m0 + 1] = max(pk[m0 + 1], pk[m0])
-            pk[m0] = 0.0
-        bm = np.concatenate([[ceiling], np.maximum(ceiling, pk), [ceiling]])     # bm[b + 1] = block b
-        db = np.concatenate([[0.0], dpk, [0.0]])
-        pe = np.concatenate([[False], pk + dpk > ceiling, [False]])              # the GPU could see this block above the ceiling
-        # per block b (index b + 1 of bm): gain at its start and end, their bound, whether the GPU could ramp at all
-        Ms, Me = np.maximum(bm[:-2], bm[1:-1]), np.maximum(bm[1:-1], bm[2:])
-        dMs, dMe = np.maximum(db[:-2], db[1:-1]), np.maximum(db[1:-1], db[2:])
-        s0, s1 = ceiling / Ms, ceiling / Me
-        ds = np.maximum(ceiling * dMs / (Ms * np.maximum(Ms - dMs, ceiling)), ceiling * dMe / (Me * np.maximum(Me - dMe, ceiling))) + 6 * U
-        eng = pe[:-2] | pe[1:-1] | pe[2:]
-        scale = s0[rel] + (g % B) * ((s1 - s0) / B)[rel]
-        del g
-        out = y * scale[:, None]
-        dsp, ep = ds[rel][:, None], eng[rel][:, None]
-        bound = np.where(ep, by * (scale[:, None] + dsp) + np.abs(y) * dsp + U * np.abs(out), by)
+        out, bound = limiter_ref(y, by, limiter_block, ceiling, stream_pos0, move_peak=m0 if mutate == "peak" else None)
     return out[:n], bound[:n], (snr_d, snr_s, snr_b)
+
+
+def limiter_ref(y, by, block, ceiling, stream_pos0, move_peak=None):
+    """the limiter on y [n][C] (bound by) at stream positions stream_pos0 + i, on the stream's grid of `block`-frame blocks: the
+    blocks before and after y count as the ceiling.  move_peak = b: block b's peak is given to block b + 1 (test_bound_is_sharp)."""
+    B = block
+    g = stream_pos0 + np.arange(len(y), dtype=np.int64)
+    rel = g // B - stream_pos0 // B
+    starts = np.concatenate([[0], np.flatnonzero(np.diff(rel)) + 1])
+    pk = np.maximum.reduceat(np.abs(y).max(axis=1), starts)
+    dpk = np.maximum.reduceat(by.max(axis=1), starts)
+    if move_peak is not None and move_peak + 1 < len(pk):
+        pk[move_peak + 1] = max(pk[move_peak + 1], pk[move_peak])
+        pk[move_peak] = 0.0
+    bm = np.concatenate([[ceiling], np.maximum(ceiling, pk), [ceiling]])     # bm[b + 1] = block b
+    db = np.concatenate([[0.0], dpk, [0.0]])
+    pe = np.concatenate([[False], pk + dpk > ceiling, [False]])              # the GPU could see this block above the ceiling
+    # per block b (index b + 1 of bm): gain at its start and end, their bound, whether the GPU could ramp at all
+    Ms, Me = np.maximum(bm[:-2], bm[1:-1]), np.maximum(bm[1:-1], bm[2:])
+    dMs, dMe = np.maximum(db[:-2], db[1:-1]), np.maximum(db[1:-1], db[2:])
+    s0, s1 = ceiling / Ms, ceiling / Me
+    ds = np.maximum(ceiling * dMs / (Ms * np.maximum(Ms - dMs, ceiling)), ceiling * dMe / (Me * np.maximum(Me - dMe, ceiling))) + 6 * U
+    eng = pe[:-2] | pe[1:-1] | pe[2:]
+    scale = s0[rel] + (g % B) * ((s1 - s0) / B)[rel]
+    del g
+    out = y * scale[:, None]
+    dsp, ep = ds[rel][:, None], eng[rel][:, None]
+    bound = np.where(ep, by * (scale[:, None] + dsp) + np.abs(y) * dsp + U * np.abs(out), by)
+    return out, bound
 
 
 def embed_ref_offset(x, fm, z, pad=250, wd=0.01, limiter_block=44100, ceiling=CEIL, **kw):
@@ -580,11 +603,15 @@ def test_batch(mode):
             check_s16("batch s16 item %d" % i, o, w, b)
         return
     if mode == "rates":
+        from test_gpu_resample_ref import add_rates_ref
         rates = [RATE if i % 2 == 0 else 48000 for i in range(len(pcms))]
         outs = H.add_batch_rates(pcms, pays, rates)
         for i, (o, (w, b, _)) in enumerate(zip(outs, refs)):
             if rates[i] == RATE:
                 check("batch rates item %d (44.1 kHz)" % i, o, w, b)
+            else:
+                w, b, _, _ = add_rates_ref(pcms[i], rates[i], oracle_fm(O.Key(bytes(keys[i])), pays[i]))
+                check("batch rates item %d (48 kHz)" % i, o, w, b)
         return
     kw = dict(zero_frames=zs) if mode in ("offsets", "keys") else {}
     if mode == "keys":
